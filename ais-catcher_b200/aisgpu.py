@@ -8,7 +8,7 @@ import os
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("AISGPU_LIB") or os.path.join(HERE, "libaisgpu.so")  # AISGPU_LIB: A/B of two builds of the library in one gpurun call
+LIB_PATH = os.environ.get("AISGPU_LIB") or os.path.join(HERE, "libaisgpu.so")  # AISGPU_LIB: A/B of two builds of the library on one machine
 
 MODEL_STANDARD, MODEL_BASE, MODEL_DEFAULT, MODEL_CHALLENGER, MODEL_V2 = 0, 1, 2, 4, 11
 FMT_CF32, FMT_CU8, FMT_CS8, FMT_CS16 = 0, 1, 2, 3

@@ -103,7 +103,7 @@ struct aisgpu_handle {
 	int max_n48 = 0;
 	int fe_warps = 4, fe_tile = 0, fe_ctas = 4096;
 	int fe_st = 1, st_L = 0, st_ring = 0, st_kmax = 7; // AISGPU_FE_ST=0 disables the per-thread streaming kernel; AISGPU_ST_L: lanes per stream (0: the launcher plans); AISGPU_ST_NB: ring depth 3 | 5 (0: per chain)
-	int cf_rows = 8; // AISGPU_CF_ROWS: rows per CTA of the fused CGF kernel (4 or 8); 8 halves the chain warp's instructions: 0.427 vs 0.433 ms per step (ModelDefault, bench.py A/B, twice)
+	int cf_rows = 8; // AISGPU_CF_ROWS: rows per CTA of the fused CGF kernel (4 or 8); 8 halves the chain warp's instructions (chosen on the previous target; not re-measured on the H100)
 	int dec_rpw = 6, decoder = 3; // rows per warp / which decoder kernel // front-end launch shape (tunable through AISGPU_FE_WARPS / _TILE / _CTAS)
 	// fe_stream: front end + input history; stream: everything behind the 48 kHz buffers (the stream handed to callers
 	// for timing).  The front end of submit c+1 overlaps the back end of submit c; Cbuf is double buffered for that.
@@ -378,7 +378,7 @@ int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int 
 	if (tile != p.tile) layout_frontend(p, h->k, tile);
 	h->tile = tile;
 	const int B = h->cfg.n_streams;
-	int n_seg = (h->fe_ctas + B - 1) / B; // enough CTAs for several waves over 148 SMs
+	int n_seg = (h->fe_ctas + B - 1) / B; // enough CTAs for several waves over the SMs
 	int tiles_total = (N + tile - 1) / tile;
 	if (n_seg > tiles_total) n_seg = tiles_total;
 	if (n_seg < 1) n_seg = 1;
@@ -405,13 +405,9 @@ int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int 
 		p.in = dev_in;
 		p.st_B = B;
 		p.st_first = h->chunk == 0 ? 1 : 0;
-		// CF32 launch shape, measured live at 1024 x 131072 (gpurun probes r2b-1 .. r2b-9, per-block step times):
-		//   ring of 3 chunks (104 KB per CTA) + ONE balanced wave (the planner, one CTA per SM: L = 18, 144 CTAs):
-		//       ModelStandard 0.266 ms, ModelDefault 0.43 ms, Challenger 0.54 ms  <- shipped for every chain
-		//   ring of 5 (174 KB) + power-of-two split L = 32 (256 CTAs, 1.73 waves; the round-2a shape):   0.294 / 0.475 / 0.56 ms
-		//   ring of 5 + L = 18: 0.302-0.310 / 0.455 ms;   ring of 3 + L = 32: 0.311 ms;   ring of 3, two CTAs per SM (L = 37): 0.292-0.313 / 0.446 ms
+		// CF32 launch shape: ring of 3 chunks (104 KB per CTA) + ONE balanced wave (the planner, one CTA per SM), chosen over rings
+		// of 5 and power-of-two lane splits on live step times at 1024 x 131072 on the previous target (not re-measured on the H100).
 		// The smaller ring leaves 123 KB of the SM to the back-end CTAs that run beside the front end of the next submit.
-		// (Throttling the FM kernel's occupancy with unused shared memory so that it cannot crowd the front end: 0.33-0.38 ms, worse.)
 		const int L = h->st_L;
 		p.st_ring = h->st_ring ? h->st_ring : 3;
 		p.st_cap = (h->in_fmt == 0 && !h->fp_ds) ? 1 : 0; // the integer formats run one-warp CTAs, as many per SM as fit
@@ -863,8 +859,8 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 			if (h->fe_st && h->kA >= 3 && h->kA <= 5 && ((stride * h->obps) % 16) == 0 && (((size_t)dev_in) % 16) == 0) {
 				pp.st_B = B;
 				// the decimation in front of the resampler runs the same launch shape as the front end proper (four-warp CTAs, ring of 3, one
-				// balanced wave): configs[2] (4096 x 65536 @6 MSPS) 0.70 -> 0.66 ms per step, 1024 x 393216 @6 MSPS 0.91 -> 0.83 ms against
-				// one-warp CTAs with 16-sample chunks
+				// balanced wave), which was faster than one-warp CTAs with 16-sample chunks at 6 MSPS on the previous target (not re-measured
+				// on the H100)
 				pp.st_ring = h->st_ring ? h->st_ring : 3;
 				pp.st_cap = h->cfg.format == 0 ? 1 : 0;
 				const cudaError_t e = launch_frontend_stream(pp, h->cfg.format, h->kA, true, h->st_L, h->fe_stream);
@@ -1181,8 +1177,8 @@ static int create_impl(aisgpu_handle *h) {
 #else
 	h->fe_warps = 4;
 #endif
-	// rows per warp of the decoder kernel, measured per chain: the coherent chain 1; the FM chain 3 with the round-2b front-end shape
-	// (bench.py A/B, three pairs: 0.266 / 0.276 / 0.263 ms per step against 0.273 / 0.278 / 0.278 with 6 rows per warp)
+	// rows per warp of the decoder kernel, chosen per chain on the previous target (not re-measured on the H100): the coherent
+	// chain 1; the FM chain 3 with the current front-end shape (slightly faster than 6 rows per warp)
 	h->dec_rpw = c.model == AISGPU_MODEL_DEFAULT ? 1 : (c.model == AISGPU_MODEL_STANDARD ? 3 : 6);
 	if (const char *e = getenv("AISGPU_DEC_RPW")) {
 		h->dec_rpw = atoi(e);
@@ -1204,7 +1200,7 @@ static int create_impl(aisgpu_handle *h) {
 	if (const char *e = getenv("AISGPU_FE_CTAS")) h->fe_ctas = std::max(1, atoi(e));
 	int ndev = 0;
 	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
-		h->err = "no CUDA device (the B200 path has no CPU fallback)";
+		h->err = "no CUDA device (the CUDA path has no CPU fallback)";
 		return AISGPU_ENODEV;
 	}
 	if (c.device < 0 || c.device >= ndev) {
@@ -1224,10 +1220,10 @@ static int create_impl(aisgpu_handle *h) {
 	h->be_streams[0] = h->be_streams[1] = h->stream;
 	{
 		const char *e = getenv("AISGPU_BE_PIPE");
-		// Overlapping the stages of consecutive submits over two back-end streams pays +6 % for the FM chain.  For the coherent chain
-		// it is what keeps the step time stable: with one back-end stream the run can lock into a serial pattern (front end c+1 starved
-		// while back end c runs, back end c+1 then waiting for it) -- 0.80 ms per step (or 0.90 ms with one stream priority) instead of
-		// 0.55 ms at 1024 x 131072 @1536K, both patterns self-sustaining from the first submits on (profiles/r2_sweeps.jsonl, probe12/13).
+		// Overlapping the stages of consecutive submits over two back-end streams paid a few per cent for the FM chain on the previous
+		// target.  For the coherent chain it is what keeps the step time stable: with one back-end stream the run can lock into a serial
+		// pattern (front end c+1 starved while back end c runs, back end c+1 then waiting for it) that costs about half again per step,
+		// self-sustaining from the first submits on (tools/default_probe.py shows which pattern a process lands in).
 		const bool pipe = (e ? atoi(e) != 0 : (c.model == AISGPU_MODEL_STANDARD || c.model == AISGPU_MODEL_DEFAULT || c.model == AISGPU_MODEL_CHALLENGER)) && !c.enable_taps &&
 						  c.model != AISGPU_MODEL_BASE && c.model != AISGPU_MODEL_V2;
 		if (pipe) CU(cudaStreamCreateWithPriority(&h->be_streams[1], cudaStreamNonBlocking, prio_hi));

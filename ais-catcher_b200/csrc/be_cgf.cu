@@ -101,11 +101,11 @@ __constant__ float c_taps_coherent[FIRC_T]; // FilterComplex 17 taps (Filters.h:
 // ---------------------------------------------------------------------------------------------
 // K2bc: the derotation phasor chain, output[i] *= rot and FilterComplex 17 taps in ONE kernel (DSP.cpp:457-465, 215-246).
 // The chain rot *= rot_step is strictly sequential per row (4096 dependent complex products per submit at the bench
-// shape: ~17 us is the floor for the whole stage), everything else is parallel.  A CTA owns CF_ROWS rows: warp 0 runs
+// shape: their latency is the floor for the whole stage), everything else is parallel.  A CTA owns CF_ROWS rows: warp 0 runs
 // the chains, one lane per row, CF_T steps ahead into a double-buffered shared tile; meanwhile the two consumer warps
 // derotate the previous tile (coalesced loads of the 48 kHz samples, requested one tile ahead), and run the FIR out of a
-// shared ring that keeps the 16-sample history.  The phasors never travel through HBM (round 1 wrote them out, 67 MB per submit, and read them back).  FIR: products by scalar FMUL, the (re, im) accumulation by one packed FADD2 --
-// ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2, a scalar product feeding a packed add stays two roundings.
+// shared ring that keeps the 16-sample history.  The phasors never travel through HBM (an earlier version wrote them out, 67 MB per submit, and read them back).  FIR: products
+// by scalar __fmul_rn, the (re, im) accumulation by padd (two scalar __fadd_rn): two roundings per tap, as in the reference.
 // ---------------------------------------------------------------------------------------------
 constexpr int CF_T = 64;               // samples per tile and row (a 512-block = 8 tiles)
 // CF_ROWS rows per CTA, CF_CONS = CF_ROWS / 2 consumer warps (four outputs per thread and tile): 4 rows -> 512 CTAs at 2048 rows

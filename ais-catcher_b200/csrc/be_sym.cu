@@ -164,9 +164,9 @@ __global__ void __launch_bounds__(PS_THREADS) k_phase_search(const K3Params p) {
 //   * the only sequential part left is  i0 = (max_idx - 1) & 15; max_idx = (i0 + table[i0]) & 15  -- one shuffle (from the
 //     lane holding entry i0) and integer work that no longer waits for floating-point results of the same symbol;
 //   * the lane that holds hypothesis max_idx contributes the demodulated bit (its decisions 3 and 4 symbols ago, XORed).
-// Measured alternatives at 1024 x 131072 @1536K: one hypothesis per lane (16 lanes per instance, 5120 warps) 340 us; this kernel
-// (4 lanes, 1280 warps) 212 us; eight hypotheses per lane (2 lanes, 640 warps, 28 % fewer warp instructions) 232 us -- below
-// four lanes the per-warp dependency chains are no longer hidden by other warps (2.2 warps per scheduler here).
+// Alternatives measured at 1024 x 131072 @1536K on the previous target (not re-measured on the H100): one hypothesis per lane
+// (16 lanes per instance, 5120 warps) and eight hypotheses per lane (2 lanes, 640 warps, fewer warp instructions) were both
+// slower than this kernel's 4 lanes / 1280 warps -- below four lanes the per-warp dependency chains are no longer hidden by other warps.
 // 2.7x fewer warp instructions per (instance, symbol) than one hypothesis per lane, three shuffles (one of them on the
 // sequential chain) instead of four dependent ones.  Demod::PhaseSearch (PS_EMA off) keeps the one-hypothesis-per-lane kernel above.
 // ---------------------------------------------------------------------------------------------
@@ -246,8 +246,7 @@ __global__ void __launch_bounds__(32) k_phase_search_ema4(const K3Params p) {
 			float re = (rot & 1) ? -x.y : x.x, im = (rot & 1) ? x.x : x.y;
 			if (rot & 2) { re = -re; im = -im; }
 			rot = (rot + 1) & 3;
-			// products by packed FMUL2 (two hypotheses per instruction), sums by scalar FADD: a packed mul feeding a packed add would
-			// be contracted into FFMA2 by ptxas, a packed mul feeding scalar adds keeps both roundings (checked in SASS)
+			// products of two hypotheses per pmul (two scalar __fmul_rn), then the sums: every product and sum rounded separately
 			const c64 re2 = pack2(re, re), im2 = pack2(im, im);
 			const float2 a01 = unpack2(pmul(re2, cj01)), a23 = unpack2(pmul(re2, cj23));
 			const float2 b01 = unpack2(pmul(im2, sj01)), b23 = unpack2(pmul(im2, sj23));
@@ -413,7 +412,7 @@ __global__ void __launch_bounds__(32, 28) k_phase_search_ema4b(const K3Params p)
 		const float X = (r & 1) ? x.y : x.x, Y = (r & 1) ? x.x : x.y;
 		const bool nA = r == 1 || r == 2, nB = r >= 2;
 		const c64 X2 = pack2(X, X), Y2 = pack2(Y, Y);
-		// products by packed FMUL2, sums by scalar FADD (a packed mul feeding a packed add would be contracted into FFMA2 by ptxas)
+		// products two hypotheses per pmul, then the sums, each rounded separately (__fmul_rn / __fadd_rn, never an FMA)
 		const float2 a01 = unpack2(pmul(X2, nA ? cN01 : cP01)), a23 = unpack2(pmul(X2, nA ? cN23 : cP23));
 		const float2 b01 = unpack2(pmul(Y2, nB ? sN01 : sP01)), b23 = unpack2(pmul(Y2, nB ? sN23 : sP23));
 		const float t0 = __fadd_rn(a01.x, b01.x), t1 = __fadd_rn(a01.y, b01.y), t2 = __fadd_rn(a23.x, b23.x), t3 = __fadd_rn(a23.y, b23.y);
@@ -1395,7 +1394,7 @@ cudaError_t sym_init(const float *ps_cos8, const float *ps_sin8, const uint32_t 
 cudaError_t launch_phase_search(const K3Params &p, cudaStream_t s) {
 	if (p.ps_ema) { // four hypotheses per lane (PhaseSearchEMA only)
 		const unsigned grid = (unsigned)(((long long)p.rows * 5 + PS2_INST - 1) / PS2_INST);
-		static const bool old_kernel = getenv("AISGPU_PS_OLD") != nullptr; // A/B switch of this round's measurements
+		static const bool old_kernel = getenv("AISGPU_PS_OLD") != nullptr; // A/B switch against the earlier kernel
 		if (old_kernel) k_phase_search_ema4<<<grid, 32, 0, s>>>(p);
 		else switch (p.ps_rot0 & 3) { // (1j)^rot at the first symbol of the submit
 			case 0: k_phase_search_ema4b<0><<<grid, 32, 0, s>>>(p); break;

@@ -146,19 +146,18 @@ __device__ __forceinline__ float fd_atan2f_common(float y, float x) {
 	return __uint_as_float(__float_as_uint(v) ^ (~hy & 0x80000000u));
 }
 
-// ---- packed binary32 pairs (SASS FADD2 / FMUL2): one instruction rounds both lanes exactly like two scalar
-// ---- __fadd_rn / __fmul_rn (verified bit-for-bit on 1.6e7 patterns incl. denormals, tools/microbench_f32x2.cu);
-// ---- a complex sample is one 64-bit register pair, so a complex add is ONE issue slot instead of two.
+// ---- binary32 pairs: a complex sample is one 64-bit register pair.  sm_90 has no packed FP32 instruction, so a pair
+// ---- operation is two scalar __fadd_rn / __fmul_rn (each lane rounded on its own; never contracted into an FMA).
 typedef unsigned long long c64;
+__device__ __forceinline__ float2 unpack2(c64 v);
+__device__ __forceinline__ c64 pack2(float x, float y);
 __device__ __forceinline__ c64 padd(c64 a, c64 b) {
-	c64 r;
-	asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-	return r;
+	const float2 x = unpack2(a), y = unpack2(b);
+	return pack2(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y));
 }
 __device__ __forceinline__ c64 pmul(c64 a, c64 b) {
-	c64 r;
-	asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-	return r;
+	const float2 x = unpack2(a), y = unpack2(b);
+	return pack2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
 }
 __device__ __forceinline__ c64 pack2(float x, float y) {
 	c64 r;

@@ -10,10 +10,10 @@ namespace aisgpu {
 // K1'': the front end as the reference writes it -- a per-sample streaming pipeline with its state in registers --
 // run by every THREAD on its own sub-segment of a stream.  A lane walks [a - P, a + S): the first P samples only warm
 // the state up from zero (each CIC stage is a pure function of its last six inputs, see k_frontend), after that every
-// 2^(K+1) inputs yield one 48 kHz sample per channel.  Per input pair a Downsample2CIC5 stage costs 9 packed adds and
-// one packed multiply (DSP.cpp:93-117, literally: r_k = z; z += h_k / h_k = z; z += r_k) and nothing goes through shared
-// memory between stages (ptxas fuses the exact 1/32 scaling of a stage with the first add of the next one into FFMA2;
-// a power-of-two factor makes that bit-identical to the separate multiply unless a value is subnormal); shared memory only stages the input: the warp fetches the next 16 samples of all 32 lanes with
+// 2^(K+1) inputs yield one 48 kHz sample per channel.  Per input pair a Downsample2CIC5 stage costs 9 complex adds and
+// one complex multiply (DSP.cpp:93-117, literally: r_k = z; z += h_k / h_k = z; z += r_k), each a pair of scalar
+// __fadd_rn / __fmul_rn (exact.cuh: rounded separately, never contracted into an FMA, subnormals kept), and nothing goes
+// through shared memory between stages; shared memory only stages the input: the warp fetches the next 16 samples of all 32 lanes with
 // coalesced 16-byte cp.async copies (raw format, converted when read) into a ring, four chunks ahead.
 // ---------------------------------------------------------------------------------------------
 struct Cic5 { c64 h0, h1, h2, h3, h4; };
@@ -115,8 +115,8 @@ __device__ __forceinline__ void st_read_pair(const unsigned char *slot, int j, c
 }
 
 // ST_WARPS: warps per CTA (independent of each other).  One-warp CTAs with a ring of 6 chunks (27.6 KB for CF32) let eight
-// CTAs share an SM and let the block scheduler spread B x st_wps warps evenly over the 148 SMs (1024 warps: 7 + 6.9 avg);
-// the 4-warp / ring-of-8 shape (147 KB per CTA, one CTA per SM, 1.73 waves at 1024 warps) is the round-1 shape, kept for A/B.
+// CTAs share an SM and let the block scheduler spread B x st_wps warps evenly over the SMs (1024 warps on 132: 7.8 avg);
+// the 4-warp / ring-of-8 shape (147 KB per CTA, one CTA per SM) is the earlier shape, kept for A/B.
 // ST_G: samples a lane fetches per visit of its sub-segment.  Every lane is an independent sequential stream for DRAM (1024 warps
 // = 32768 streams, far more than there are banks), so the bytes per visit decide the row-buffer locality: 16 samples = one
 // 128-byte line per visit, 64 samples = four consecutive lines.
@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(ST_WARPS * 32) k_frontend_st(const FeParams p)
 	const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
 	// Lane mapping: global lane g owns sub-segment (g % L) of stream (g / L).  A stream's nss = q * L + r super-steps are split
 	// unevenly -- the first L - r lanes take q, the last r take q + 1 -- so that L need not divide the block: the host picks L such
-	// that all CTAs are resident at once (one wave over the 148 SMs) with the longest sub-segments that allow (launch_st_one).
+	// that all CTAs are resident at once (one wave over the SMs) with the longest sub-segments that allow (launch_st_one).
 	const long long g0 = ((long long)blockIdx.x * ST_WARPS + wib) * 32;
 	const int L = p.st_L;
 	if (g0 >= (long long)p.st_B * L) return; // whole warp
@@ -210,11 +210,9 @@ __global__ void __launch_bounds__(ST_WARPS * 32) k_frontend_st(const FeParams p)
 		rt_n1[i] = PRE ? make_float2(0.f, 0.f) : __ldg(rot_g + i);
 		rt_n2[i] = PRE ? make_float2(0.f, 0.f) : __ldg(rot_g + (n_super > 1 ? N96 : 0) + i);
 	}
-	// Measured on this loop and dropped (bench.py A/B against the previous build of the library on one box, AISGPU_LIB):
-	//   two super-steps per trip (the ~60 register moves at the back edge paid once per two: 7 % fewer instructions, but 178 instead of
-	//   164 registers and twice the code): live step 0.288 vs 0.269 ms; the droop filter selected instead of branched (30 fewer
-	//   instructions per super-step): 0.277 vs 0.278 ms; __maxnreg__(152) (three spilled pairs): 0.338 ms; the chunk loop below rolled
-	//   (kernel 1136 instead of 1552 instructions, but the state moves are paid per chunk: +21 % executed): 0.285 vs 0.269 ms.
+	// Tried on this loop on the previous target and dropped, each slower live (not re-measured on the H100): two super-steps per
+	//   trip (fewer back-edge register moves, but more registers and twice the code); the droop filter selected instead of branched;
+	//   a register cap that spills; the chunk loop below rolled (smaller kernel, but the state moves are paid per chunk).
 	for (int ss = 0; ss < n_super; ss++) {
 		float2 rt[N96];
 #pragma unroll
@@ -281,7 +279,7 @@ __global__ void __launch_bounds__(ST_WARPS * 32) k_frontend_st(const FeParams p)
 					if (live && !PRE) { // y is 96 kHz sample idx (0..N96-1) of the super-step
 						c64 x = y;
 						if (p.use_fdc) { // FilterComplex3Tap: alpha * (h1 + x) + h2 * beta (DSP.cpp:283-293)
-							// scalar intrinsics: ptxas would contract a packed mul + add pair into FFMA2 here, and these products are not exact
+							// FilterComplex3Tap's own operation order, each product and sum rounded separately
 							const float2 h1 = unpack2(fd1), h2 = unpack2(fd2), yv = unpack2(y);
 							const float tx = __fadd_rn(h1.x, yv.x), ty = __fadd_rn(h1.y, yv.y);
 							x = pack2(__fadd_rn(__fmul_rn(p.fdc_alpha, tx), __fmul_rn(h2.x, p.fdc_beta)),
@@ -326,10 +324,10 @@ __global__ void __launch_bounds__(ST_WARPS * 32) k_frontend_st(const FeParams p)
 
 // ---- launch entry point of one sample format (instantiated by fe_stream_f<FMT>.cu) ----
 // Lanes per stream: the cost of a launch is modelled as waves x (super-steps per lane, warm-up included), a wave being what
-// the SMs hold at once (148 x resident CTAs of this shape).  Sub-segments shorter than `min_ratio` warm-ups are not considered;
+// the SMs hold at once (SM count x resident CTAs of this shape).  Sub-segments shorter than `min_ratio` warm-ups are not considered;
 // among (nearly) equal costs the fewest lanes win -- every lane re-reads P samples of warm-up.
-// 1024 streams x 2048 super-steps, four-warp CTAs, one per SM: L = 18 (144 CTAs, 114 + 6 super-steps) against 140 for the
-// power-of-two split L = 32 (256 CTAs = 1.73 waves of 64 + 6).
+// 1024 streams x 2048 super-steps, four-warp CTAs, one per SM on 132 SMs: L = 16 (128 CTAs, 128 + 6 super-steps) against
+// 140 for the split L = 32 (256 CTAs = 2 waves of 64 + 6).
 static inline bool st_plan(long long B, int nss, int warm, int wpc, int slots, int min_ratio, int forced_L, int &L, int &q, int &r) {
 	const int q_min = warm * min_ratio > 0 ? warm * min_ratio : 1;
 	if (nss < q_min) return false;

@@ -12,13 +12,11 @@ cudaError_t launch_frontend_stream(const FeParams &p, int fmt, int k, bool pre, 
 			if (p.st_ring == 3) return launch_frontend_stream_shape<0, 32, 3, 4>(p, k, true, forced_L, s);
 			return launch_frontend_stream_shape<0, 16, 6, 1>(p, k, true, forced_L, s);
 		}
-		// 32-sample visits, ring of 5, four-warp CTAs (one CTA per SM): the best of the shapes measured -- 16 / 32 / 64 samples per
-		// visit, one-, two- and four-warp CTAs, rings of 2 .. 8 chunks with one to eight CTAs sharing an SM (profiles/r2_sweeps.jsonl):
+		// 32-sample visits, ring of 5, four-warp CTAs (one CTA per SM): the best of the shapes measured on the previous target -- 16 / 32 / 64 samples per
+		// visit, one-, two- and four-warp CTAs, rings of 2 .. 8 chunks with one to eight CTAs sharing an SM:
 		// more resident warps never helped, the kernel is bound by what DRAM delivers for 32768 concurrent sequential streams.
-		// Round 2b: rings of 3 / 4 chunks (104 / 139 KB, room for back-end CTAs next to the front end's) change the live step by
-		// less than +-2 % for every model (gpurun probes 3: ModelDefault 0.446 / 0.455 vs 0.447 ms, ModelStandard 0.292 vs 0.293 ms)
 		// ring of 3 (104 KB per CTA instead of 174 KB): what the coherent chains run with -- their back-end CTAs (the FFT estimate
-		// alone takes 67 KB) then fit on the SM beside the front end's: 0.43 vs 0.455-0.48 ms per step (ModelDefault, 1024 x 131072)
+		// alone takes 67 KB) then fit on the SM beside the front end's.
 		if (p.st_ring == 3) return launch_frontend_stream_shape<0, 32, 3, 4>(p, k, false, forced_L, s);
 		return launch_frontend_stream_shape<0, 32, 5, 4>(p, k, false, forced_L, s);
 	case 1: return launch_frontend_stream_shape<1, 16, 8, 1>(p, k, pre, forced_L, s);

@@ -1,4 +1,4 @@
-// ModelGPU.h -- the B200 engine as one more AIS::Model of the reference application.
+// ModelGPU.h -- the H100 engine as one more AIS::Model of the reference application.
 //
 // Header-only C++11 adapter, compiled against the reference's own headers where they lie (add the reference's
 // Source/* directories to the include path; nothing of the reference is copied here) and linked with libaisgpu.so
@@ -103,7 +103,7 @@ public:
 		cfg.model = kind;
 		cfg.n_streams = 1;
 		frames.resize(64);
-		setName(kind == AISGPU_MODEL_DEFAULT ? "AIS engine B200 (coherent)" : (kind == AISGPU_MODEL_STANDARD ? "AIS engine B200 (FM)" : "AIS engine B200 (FM/PLL)"));
+		setName(kind == AISGPU_MODEL_DEFAULT ? "AIS engine H100 (coherent)" : (kind == AISGPU_MODEL_STANDARD ? "AIS engine H100 (FM)" : "AIS engine H100 (FM/PLL)"));
 	}
 	~ModelGPU() override { aisgpu_destroy(engine); }
 

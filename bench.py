@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- IQ MSamples/s through the full two-channel AIS demodulation chain on B200.
+"""bench.py -- IQ MSamples/s through the full two-channel AIS demodulation chain on H100.
 
 Contract: `python bench.py --gpus N --steps K --warmup W` (under torchrun for N>1) prints ONE JSON line on rank 0.
 A "step" is one submit of one batch: B streams x N complex samples (BASELINE.json configs[1]: batch=1024 synthetic
 CF32 streams @1536 kSPS, FM path = ModelStandard semantics, SURVEY.md 8d "Config 2"), inputs already resident in HBM.
   value     : whole-job complex samples/s (all ranks) with inputs resident in HBM, device-timed on the launch stream:
-              the K-step block is run `--blocks` times back to back (timed region >= 150 ms), the MEDIAN block is the
-              value, min/max go to `spread`, every rank's median to `per_rank_ms`
+              exactly K timed submits (default 300, ~150 ms), split into `--blocks` back-to-back blocks (default one); the MEDIAN per-step
+              time over the blocks is the value, min/max go to `spread`, every rank's median to `per_rank_ms`
   e2e       : the same metric through aisgpu_submit_async()/aisgpu_poll_upto() with pinned HOST buffers (H2D and the
               frame D2H inside the timed region); e2e_cu8 = the same with CU8 host input (2 B/sample)
   roofline  : front-end kernel (reads every input byte): 8 B/sample x samples per launch / its CUDA-event duration,
@@ -17,6 +17,8 @@ CF32 streams @1536 kSPS, FM path = ModelStandard semantics, SURVEY.md 8d "Config
   also      : ModelDefault on the same data, and BASELINE.json configs[2] (batch 4096 @6 MSPS, coherent chain)
   cpu_baseline : the reference's own CPU implementation (oracle/_ref fast build, shipping flags) on this box's cores
 `--impl reference` times that CPU implementation alone on the same workload shape (steady state).
+`--dump-outputs DIR` writes the frames the last timed submit completed (what aisgpu_poll hands a caller), gathered from all
+ranks with streams numbered rank * batch + stream, as DIR/<name>.npy (rank 0 writes).
 """
 import argparse
 import ctypes
@@ -57,7 +59,7 @@ def peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler(threading.Thread):
@@ -204,7 +206,7 @@ def config_dict(args, world):
     """Identical for the CUDA arm and the reference arm (the driver compares the two `config` objects key by key)."""
     return {"workload": workload_name(args), "model": args.model, "sample_rate": FS, "batch_per_gpu": args.batch,
             "chunk_samples": N_CHUNK, "resident_chunks": RESIDENT, "bytes_per_step_per_gpu": args.batch * N_CHUNK * 8,
-            "l2": "inputs_larger_than_L2 (1.07 GB per step vs 126 MB L2)", "parallelism": "streams sharded, %d rank(s)" % world}
+            "l2": "inputs_larger_than_L2 (1.07 GB per step vs 50 MB L2)", "parallelism": "streams sharded, %d rank(s)" % world}
 
 
 def run_reference_arm(args, rank, world):
@@ -242,9 +244,11 @@ def median(v):
     return s[len(s) // 2]
 
 
-def poll_streams(eng, wanted, out):
+def poll_streams(eng, wanted, out, keep_chunk=None, kept=None):
     """Drains the engine's frame queue; keeps (key, start_idx, end_idx) only for the streams in `wanted` (a set) -- the
-    ctypes structs of the other streams are never turned into Python objects.  Returns the number of frames drained."""
+    ctypes structs of the other streams are never turned into Python objects -- and, when `keep_chunk` is given, every frame
+    that submit completed as (stream, channel, nbits, start_idx, end_idx, level, ppm, payload) in the list `kept`.
+    Returns the number of frames drained."""
     import aisgpu
     batch = 8192
     buf = (aisgpu.MsgStruct * batch)()
@@ -256,10 +260,39 @@ def poll_streams(eng, wanted, out):
             break
         total += n.value
         for i in range(n.value):
+            if keep_chunk is not None and buf[i].chunk == keep_chunk:
+                f = buf[i]
+                kept.append((f.stream, f.channel[0], f.nbits, f.start_idx, f.end_idx, f.level, f.ppm, bytes(f.data[:(f.nbits + 7) // 8])))
             if buf[i].stream in wanted:
                 m = aisgpu.Msg(buf[i])
                 out[m.stream].append((m.key(), m.start_idx, m.end_idx))
     return total
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_frames(frames, d):
+    """Writes frames (tuples as poll_streams keeps them) as DIR/frames_<field>.npy, one row per frame in (stream, channel,
+    start) order: counters as float64 (exact below 2^53), level/ppm as float32, payload bytes (zero past nbits) as float32
+    [n][140].  Above DUMP_BYTES in all, a fixed seeded sample of the frames is written instead."""
+    import numpy as np
+    frames = sorted(frames, key=lambda f: (f[0], f[1], f[3], f[4], f[2]))
+    per_frame = 5 * 8 + 2 * 4 + 140 * 4
+    if len(frames) * per_frame > DUMP_BYTES:
+        keep = np.random.default_rng(0).choice(len(frames), size=DUMP_BYTES // per_frame, replace=False)
+        frames = [frames[i] for i in sorted(keep)]
+    payload = np.zeros((len(frames), 140), dtype=np.float32)
+    for i, f in enumerate(frames):
+        payload[i, :len(f[7])] = np.frombuffer(f[7], dtype=np.uint8)
+    cols = list(zip(*frames)) if frames else [()] * 8
+    out = {"frames_" + name: np.array(cols[j], dtype=np.float32 if name in ("level", "ppm") else np.float64)
+           for j, name in enumerate(("stream", "channel", "nbits", "start_idx", "end_idx", "level", "ppm"))}
+    out["frames_payload"] = payload
+    os.makedirs(d, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(d, name + ".npy"), a)
+    return len(frames)
 
 
 def oracle_check(streams, fetch_chunk, n_chunks, got, model, fs, fmt=0, ps_ema=True):
@@ -301,18 +334,21 @@ def oracle_check(streams, fetch_chunk, n_chunks, got, model, fs, fmt=0, ps_ema=T
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=300)  # about 150 ms of timed region at the default shape
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200")
+    ap.add_argument("--impl", default="cuda")
     ap.add_argument("--model", type=int, default=0, help="0 ModelStandard (FM path, configs[1]), 2 ModelDefault, 1 ModelBase")
     ap.add_argument("--batch", type=int, default=BATCH)
-    ap.add_argument("--blocks", type=int, default=25, help="the K-step block is timed this many times; the median block is reported")
+    ap.add_argument("--blocks", type=int, default=1, help="the K timed steps are split into this many back-to-back blocks; the median per-step time is reported")
     ap.add_argument("--e2e-steps", type=int, default=12)
     ap.add_argument("--parity-streams", type=int, default=32)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-also", action="store_true", help="skip the ModelDefault / configs[2] side measurements")
     ap.add_argument("--no-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the frames of the last timed step (all ranks, streams numbered "
+                    "rank * batch + stream) as DIR/<name>.npy; rank 0 writes")
     args = ap.parse_args()
+    args.blocks = max(1, min(args.blocks, args.steps))
     args.warmup = max(args.warmup, 3) if args.impl != "reference" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -361,8 +397,10 @@ def main():
         torch.cuda.synchronize()
 
     def timed_blocks(eng, xin, n, warmup, steps, blocks, first=0):
-        """`blocks` back-to-back blocks of `steps` submits, each block bracketed by CUDA events on the engine's stream
-        (aisgpu_join makes that stream wait for every internal stream).  Returns per-block ms and the submit count."""
+        """`blocks` back-to-back blocks of submits, `steps` in all (as even as possible), each block bracketed by CUDA events
+        on the engine's stream (aisgpu_join makes that stream wait for every internal stream).  Returns the ms per step of
+        every block, the ms of the whole timed region and the submit count."""
+        sizes = [steps // blocks + (1 if b < steps % blocks else 0) for b in range(blocks)]
         est = torch.cuda.ExternalStream(eng.cuda_stream(), device=dev)
         nres = xin.shape[0]
         i = first
@@ -374,13 +412,13 @@ def main():
         eng.join()
         evs[0].record(est)
         for b in range(blocks):
-            for _ in range(steps):
+            for _ in range(sizes[b]):
                 eng.submit_device(xin[i % nres].data_ptr(), n, n)
                 i += 1
             eng.join()
             evs[b + 1].record(est)
         evs[-1].synchronize()
-        return [evs[b].elapsed_time(evs[b + 1]) for b in range(blocks)], i
+        return [evs[b].elapsed_time(evs[b + 1]) / sizes[b] for b in range(blocks)], evs[0].elapsed_time(evs[-1]), i
 
     # ---- the timed engine; the sampled streams' frames are kept for the parity check ----
     eng = aisgpu.Engine(model=args.model, sample_rate=FS, n_streams=B, max_chunk=N, device=local_rank, max_frames=1 << 20)
@@ -399,13 +437,22 @@ def main():
         dist.all_reduce(t)
     barrier()
     sampler.start()
-    blk_ms, n_sub = timed_blocks(eng, x, N, 0, args.steps, args.blocks, first=args.warmup)
+    blk_step_ms, region_ms, n_sub = timed_blocks(eng, x, N, 0, args.steps, args.blocks, first=args.warmup)
     barrier()
     sampler.stop_flag = True
-    ms = median(blk_ms)
+    ms = median(blk_step_ms) * args.steps
     launches = eng.last_launches() * args.steps
-    fe_times = eng.frontend_times(min(128, args.steps * args.blocks))
-    n_frames = poll_streams(eng, wanted, got)
+    fe_times = eng.frontend_times(min(128, args.steps))
+    last_frames = []
+    n_frames = poll_streams(eng, wanted, got, keep_chunk=n_sub - 1 if args.dump_outputs else None, kept=last_frames)
+    if args.dump_outputs:
+        last_frames = [(rank * B + f[0],) + f[1:] for f in last_frames]  # global stream index: rank r owns streams [r * B, (r + 1) * B)
+        if world > 1:
+            parts = [None] * world
+            dist.all_gather_object(parts, last_frames)
+            last_frames = [f for part in parts for f in part]
+        if rank == 0:
+            log("dumped %d frames of the last timed step to %s" % (dump_frames(last_frames, args.dump_outputs), args.dump_outputs))
     c1 = eng.counters()
     # the only collectives of the job: MAX of the device time, SUM of a few counters (NCCL over NVLink; SURVEY.md 8e)
     ms_max = shard.max_over_ranks(ms, device=dev)
@@ -416,7 +463,7 @@ def main():
         dist.all_reduce(t)
         per_rank = [float(v) for v in t.tolist()]
     delta = [a - b for a, b in zip(c1, c0)]
-    delta[2] = B * N * args.steps * args.blocks  # samples of this rank's slice (the engine counts samples per stream)
+    delta[2] = B * N * args.steps  # samples of this rank's slice (the engine counts samples per stream)
     tot = shard.gather_counts(delta, device=dev)
     # the same reduction inside the C library (aisgpu_comm_init / aisgpu_allreduce_counts: NCCL resolved with dlopen, no
     # torch on that path): the counters since engine creation, summed over the ranks -- what a C++ host would call
@@ -431,7 +478,7 @@ def main():
         local_all = shard.gather_counts(c1, device=dev)
         assert c_totals[0] == local_all[0] and c_totals[1] == local_all[1], "C-side NCCL all-reduce disagrees with torch.distributed"
     value = world * B * N * args.steps / (ms_max * 1e-3) / 1e6
-    region_ms = shard.max_over_ranks(sum(blk_ms), device=dev)
+    region_ms = shard.max_over_ranks(region_ms, device=dev)
     msgs_per_s = float(tot[1]) / (region_ms * 1e-3)
 
     # ---- parity: the sampled streams through the unmodified reference, same inputs, same chunking ----
@@ -514,8 +561,8 @@ def main():
         if args.model != 2:
             eng2 = aisgpu.Engine(model=2, sample_rate=FS, n_streams=B, max_chunk=N, device=local_rank, max_frames=1 << 20)
             got2 = {s: [] for s in sample_streams}
-            b2, n2 = timed_blocks(eng2, x, N, 3, args.steps, max(3, args.blocks // 5))
-            fe2 = eng2.frontend_times(args.steps)
+            b2, _, n2 = timed_blocks(eng2, x, N, 3, 100, 5)
+            fe2 = eng2.frontend_times(100)
             nm2 = poll_streams(eng2, wanted, got2)
             par2 = None
             if not args.no_parity:
@@ -523,34 +570,34 @@ def main():
                                     {s: got2[s] for s in sample_streams[:8]}, 2, FS)
             m2 = median(b2)
             also.append({"workload": "same data and batch, ModelDefault (coherent PhaseSearchEMA chain, the reference's default model)",
-                         "value": B * N * args.steps / (m2 * 1e-3) / 1e6, "unit": "MSamples/s (this rank)", "ms_per_step": m2 / args.steps,
-                         "whole_chain_frac": ALGO_BYTES_PER_SAMPLE * B * N / (m2 / args.steps * 1e-3) / 1e9 / peaks()[0],
+                         "value": B * N / (m2 * 1e-3) / 1e6, "unit": "MSamples/s (this rank)", "ms_per_step": m2,
+                         "whole_chain_frac": ALGO_BYTES_PER_SAMPLE * B * N / (m2 * 1e-3) / 1e9 / peaks()[0],
                          "frontend_ms": sum(fe2) / len(fe2), "frames": nm2, "parity": par2,
-                         "blocks_ms_per_step": [round(b / args.steps, 4) for b in b2]})
+                         "blocks_ms_per_step": [round(b, 4) for b in b2]})
             eng2.close()
         # SURVEY.md 8f rank 1: the V2 engine (model 11) on the same data
         engv = aisgpu.Engine(model=aisgpu.MODEL_V2, sample_rate=FS, n_streams=B, max_chunk=N, device=local_rank, max_frames=1 << 20, host_staging=False)
         gotv = {s: [] for s in sample_streams[:8]}
-        bv, nv = timed_blocks(engv, x, N, 2, 8, 3)
+        bv, _, nv = timed_blocks(engv, x, N, 2, 24, 3)
         nmv = poll_streams(engv, set(sample_streams[:8]), gotv)
         parv = None
         if not args.no_parity:
             parv = oracle_check(sample_streams[:8], lambda c: {s: x[c % R][s].cpu().numpy() for s in sample_streams[:8]}, nv, gotv, 11, FS)
         mv = median(bv)
-        also.append({"workload": "same data and batch, V2::Engine (model 11)", "value": B * N * 8 / (mv * 1e-3) / 1e6, "unit": "MSamples/s (this rank)",
-                     "ms_per_step": mv / 8, "frames": nmv, "parity": parv, "blocks_ms_per_step": [round(b / 8, 4) for b in bv]})
+        also.append({"workload": "same data and batch, V2::Engine (model 11)", "value": B * N / (mv * 1e-3) / 1e6, "unit": "MSamples/s (this rank)",
+                     "ms_per_step": mv, "frames": nmv, "parity": parv, "blocks_ms_per_step": [round(b, 4) for b in bv]})
         engv.close()
         # SURVEY.md 8f rank 3: ModelChallenger (model 4) on the same data
         engc = aisgpu.Engine(model=aisgpu.MODEL_CHALLENGER, sample_rate=FS, n_streams=B, max_chunk=N, device=local_rank, max_frames=1 << 20, host_staging=False)
         gotc = {s: [] for s in sample_streams[:8]}
-        bc, nc = timed_blocks(engc, x, N, 2, 12, 3)  # long enough blocks to show the steady state
+        bc, _, nc = timed_blocks(engc, x, N, 2, 36, 3)  # long enough blocks to show the steady state
         nmc = poll_streams(engc, set(sample_streams[:8]), gotc)
         parc = None
         if not args.no_parity:
             parc = oracle_check(sample_streams[:8], lambda c: {s: x[c % R][s].cpu().numpy() for s in sample_streams[:8]}, nc, gotc, 4, FS)
         mc = median(bc)
-        also.append({"workload": "same data and batch, ModelChallenger (model 4)", "value": B * N * 12 / (mc * 1e-3) / 1e6, "unit": "MSamples/s (this rank)",
-                     "ms_per_step": mc / 12, "frames": nmc, "parity": parc, "blocks_ms_per_step": [round(b / 12, 4) for b in bc]})
+        also.append({"workload": "same data and batch, ModelChallenger (model 4)", "value": B * N / (mc * 1e-3) / 1e6, "unit": "MSamples/s (this rank)",
+                     "ms_per_step": mc, "frames": nmc, "parity": parc, "blocks_ms_per_step": [round(b, 4) for b in bc]})
         engc.close()
         del x
         torch.cuda.empty_cache()
@@ -570,7 +617,7 @@ def main():
         for ps_ema in (True, False):
             eng3 = aisgpu.Engine(model=2, sample_rate=fs3, n_streams=B3, max_chunk=N3, ps_ema=ps_ema, device=local_rank, max_frames=1 << 20)
             got3 = {s: [] for s in s3}
-            b3, n3 = timed_blocks(eng3, x3, N3, 3, 6, 5)
+            b3, _, n3 = timed_blocks(eng3, x3, N3, 3, 30, 5)
             nm3 = poll_streams(eng3, set(s3), got3)
             par3 = None
             if not args.no_parity:
@@ -578,9 +625,9 @@ def main():
             m3 = median(b3)
             also.append({"workload": "BASELINE configs[2]: batch=4096 CF32 @6 MSPS, ModelDefault, %s, chunk %d" % (
                 "PhaseSearchEMA" if ps_ema else "PS_EMA off (Demod::PhaseSearch)", N3),
-                "value": B3 * N3 * 6 / (m3 * 1e-3) / 1e6, "unit": "MSamples/s (this rank)", "ms_per_step": m3 / 6,
-                "whole_chain_frac": 8.0 * B3 * N3 / (m3 / 6 * 1e-3) / 1e9 / peaks()[0], "frames": nm3, "parity": par3,
-                "blocks_ms_per_step": [round(b / 6, 4) for b in b3]})
+                "value": B3 * N3 / (m3 * 1e-3) / 1e6, "unit": "MSamples/s (this rank)", "ms_per_step": m3,
+                "whole_chain_frac": 8.0 * B3 * N3 / (m3 * 1e-3) / 1e9 / peaks()[0], "frames": nm3, "parity": par3,
+                "blocks_ms_per_step": [round(b, 4) for b in b3]})
             eng3.close()
         del x3
 
@@ -588,11 +635,6 @@ def main():
         peak, peak_src = peaks()
         fe_ms = sum(fe_times) / max(1, len(fe_times))
         achieved = ALGO_BYTES_PER_SAMPLE * B * N / (fe_ms * 1e-3) / 1e9
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "frontend_traffic.json")
-        if os.path.exists(tp):
-            with open(tp) as f:
-                traffic = json.load(f).get("dram_bytes_per_launch")
         cpu = None
         if not args.no_cpu:
             ref = CpuReference(uniq, args.model, B)
@@ -610,8 +652,9 @@ def main():
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": config_dict(args, world),
             "blocks": args.blocks, "timed_region_ms": region_ms,
-            "spread": {"min_ms_per_step": min(blk_ms) / args.steps, "max_ms_per_step": max(blk_ms) / args.steps,
-                       "note": "median of %d blocks of %d steps (this rank); value uses the max over ranks of the per-rank medians" % (args.blocks, args.steps)},
+            "spread": {"min_ms_per_step": min(blk_step_ms), "max_ms_per_step": max(blk_step_ms),
+                       "note": "median over %d blocks of %d steps in all (this rank); value uses the max over ranks of the per-rank medians%s" % (
+                           args.blocks, args.steps, "; a single block, so min == max (--blocks splits the steps)" if args.blocks == 1 else "")},
             "per_rank_ms": [v / args.steps for v in per_rank],
             "msgs_per_s": msgs_per_s,
             "counters_allreduce_c": c_totals,
@@ -620,10 +663,10 @@ def main():
                     "d2h_bytes_per_step": d2h, "steps": args.e2e_steps,
                     "api": "aisgpu_submit_async + aisgpu_poll_upto, two caller-owned pinned buffers"},
             "e2e_cu8": e2e_cu8,
-            "gpu_launches": launches * args.blocks,
+            "gpu_launches": launches,
             "clocks": sampler.summary(),
             "roofline": {"bound": "hbm", "kernel": "k_frontend_st", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "frontend_ms_per_launch": fe_ms, "frontend_share_of_step": fe_ms / step_ms,
                          "isolated_ms_per_launch": min(iso), "isolated_frac": ALGO_BYTES_PER_SAMPLE * B * N / (min(iso) * 1e-3) / 1e9 / peak,
                          "note": "achieved = 8 B/sample x samples per launch / live CUDA-event duration of the front-end kernel (mean of the last %d launches of the timed region) while the back end of the previous submit shares the GPU; isolated_* = the same launch alone" % len(fe_times),

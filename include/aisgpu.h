@@ -1,4 +1,4 @@
-/* aisgpu.h -- C ABI of the B200-native AIS demodulation engine.
+/* aisgpu.h -- C ABI of the H100-native AIS demodulation engine.
  *
  * Drop-in boundary for ONE hot path of jvde-github/AIS-catcher: raw IQ ->
  * decimate -> +/-25 kHz channelise -> (CGF, FIR, coherent phase search | FM

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "ais-catcher_b200"), os.path.join(ROOT, "orac
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
