@@ -12,6 +12,7 @@ LIB_PATH = os.environ.get("AISGPU_LIB") or os.path.join(HERE, "libaisgpu.so")  #
 
 MODEL_STANDARD, MODEL_BASE, MODEL_DEFAULT, MODEL_CHALLENGER, MODEL_V2 = 0, 1, 2, 4, 11
 FMT_CF32, FMT_CU8, FMT_CS8, FMT_CS16 = 0, 1, 2, 3
+MODE_AB, MODE_X = 0, 3  # aisgpu_config.channel_mode: two channels (also CD) / single channel (-c X)
 TAP_C, TAP_CGF, TAP_FIR, TAP_ROT, TAP_DEC, TAP_FM, TAP_PRE, TAP_PRE2 = 0, 1, 2, 3, 4, 5, 7, 8
 
 EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisgpu_submit", "aisgpu_submit_device",
@@ -29,7 +30,8 @@ class Config(C.Structure):
                 ("n_streams", C.c_int32), ("max_chunk_samples", C.c_int32), ("ps_ema", C.c_int32), ("afc_wide", C.c_int32),
                 ("droop", C.c_int32), ("channel_a", C.c_char), ("channel_b", C.c_char), ("station", C.c_int32),
                 ("own_mmsi", C.c_int32), ("tag_mode", C.c_uint32), ("device", C.c_int32), ("enable_taps", C.c_int32),
-                ("max_frames", C.c_int32), ("host_staging", C.c_int32), ("dsk", C.c_int32), ("fp_ds", C.c_int32), ("dd_train", C.c_float), ("dd_weight", C.c_float)]
+                ("max_frames", C.c_int32), ("host_staging", C.c_int32), ("dsk", C.c_int32), ("fp_ds", C.c_int32), ("dd_train", C.c_float), ("dd_weight", C.c_float),
+                ("channel_mode", C.c_int32)]
 
 
 class MsgStruct(C.Structure):
@@ -118,12 +120,13 @@ def load():
     return lib
 
 
-def chunk_granule(sample_rate, model=MODEL_DEFAULT, dsk=False, fp_ds=False, fmt=FMT_CF32):
+def chunk_granule(sample_rate, model=MODEL_DEFAULT, dsk=False, fp_ds=False, fmt=FMT_CF32, channel_mode=MODE_AB):
     """Granule (samples) every submit length must be a multiple of; raises with the reference's wording if unsupported."""
     lib = load()
     cfg = Config()
     lib.aisgpu_default_config(C.byref(cfg))
     cfg.sample_rate, cfg.model, cfg.dsk, cfg.fp_ds, cfg.format = sample_rate, model, int(dsk), int(fp_ds), fmt
+    cfg.channel_mode = channel_mode
     g = lib.aisgpu_chunk_granule(C.byref(cfg))
     if g <= 0:
         raise AisGpuError("rc=%d: %s" % (g, lib.aisgpu_last_error(None).decode()))
@@ -204,7 +207,7 @@ class Engine:
 
     def __init__(self, model=MODEL_DEFAULT, sample_rate=1536000, fmt=FMT_CF32, n_streams=1, max_chunk=131072,
                  ps_ema=True, afc_wide=True, droop=True, own_mmsi=-1, device=0, taps=False, max_frames=0, tag_mode=3, host_staging=True,
-                 dsk=False, fp_ds=False):
+                 dsk=False, fp_ds=False, channel_mode=MODE_AB, channels="AB"):
         self.lib = load()
         cfg = Config()
         self.lib.aisgpu_default_config(C.byref(cfg))
@@ -213,6 +216,8 @@ class Engine:
         cfg.ps_ema, cfg.afc_wide, cfg.droop = int(ps_ema), int(afc_wide), int(droop)
         cfg.own_mmsi, cfg.device, cfg.enable_taps, cfg.max_frames, cfg.tag_mode = own_mmsi, device, int(taps), max_frames, tag_mode
         cfg.host_staging, cfg.dsk, cfg.fp_ds = int(host_staging), int(dsk), int(fp_ds)
+        cfg.channel_mode = channel_mode
+        cfg.channel_a, cfg.channel_b = channels[0].encode(), channels[1].encode()  # CH1 / CH2 of buildModel
         self.cfg = cfg
         self.h = C.c_void_p()
         rc = self.lib.aisgpu_create(C.byref(cfg), C.byref(self.h))

@@ -62,6 +62,8 @@ constexpr int V2_BLK = 512; // V2::BLOCK_SIZE (V2Engine.h:30)
 constexpr int HD = 48;  // ModelChallenger: derotated samples kept in front of the new ones (FM needs 1, FIR37 36, a partial group 4)
 constexpr int HE = 8;   // room in front of new symbol-stage samples: an incomplete group of 5 (<=4)
 
+constexpr int X_GRANULE = 64; // single-channel mode: a multiple of every format's front-end lane chunk (frontend_x_granule)
+
 int bytes_per_sample(int fmt) { return fmt == AISGPU_FMT_CF32 ? 8 : (fmt == AISGPU_FMT_CS16 ? 4 : 2); }
 
 } // namespace
@@ -98,6 +100,8 @@ struct aisgpu_handle {
 	int inner_max = 0;       // longest block the front end proper can be handed
 	int use_fdc = 0;
 	int fp_ds = 0; // integer CIC front end (DS_UINT16 x 4, DSP.cpp:499-665): CU8 @1536K with -go FP_DS on
+	int xmode = 0; // single-channel mode (AISGPU_MODE_X): no Rotate, one back-end row per stream
+	int us_ratio = 2; // ceil(bucket / rate): most DSP::Upsample outputs per input sample (AB: <= 2, X: <= 4)
 	float fdc_alpha = 0, fdc_beta = 1;
 	int rows = 0;
 	int max_n48 = 0;
@@ -226,6 +230,12 @@ struct aisgpu_handle {
 
 namespace {
 
+// The back end's rows and the (stream, channel) they stand for: AB rows are stream * 2 + channel, single-channel rows are streams.
+int rows_of(const aisgpu_handle *h) { return h->xmode ? h->cfg.n_streams : 2 * h->cfg.n_streams; }
+int row_of(const aisgpu_handle *h, int stream, int channel) { return h->xmode ? stream : stream * 2 + channel; }
+int stream_of_row(const aisgpu_handle *h, int row) { return h->xmode ? row : row >> 1; }
+int channel_of_row(const aisgpu_handle *h, int row) { return h->xmode ? 0 : row & 1; }
+
 #define CU(call)                                                                                   \
 	do {                                                                                           \
 		cudaError_t e_ = (call);                                                                   \
@@ -255,9 +265,49 @@ int dalloc(aisgpu_handle *h, T **p, size_t n) {
 	return 0;
 }
 
+// Model.cpp:35-107 (mode X): bucket 48K / 96K / 192K, k = 0 .. 2 CIC stages, Upsample straight behind convert at other rates
+// (kA = 0), FilterComplex3Tap at 48 kHz behind the CIC stages (none at 48K); -go DSK / FP_DS / SOXR / SRC / MA are never read.
+int plan_frontend_x(aisgpu_handle *h) {
+	const int sr = h->cfg.sample_rate;
+	if (sr < 12000 || sr > 192000) {
+		h->err = "Model: sample rate must be between 12k and 192k (inclusive).";
+		return AISGPU_EINVAL;
+	}
+	int bucket = 48000;
+	while (bucket < sr) bucket *= 2;
+	h->pre = 0;
+	h->kA = 0;
+	h->fp_ds = 0;
+	h->in_fmt = h->cfg.format;
+	h->k = bucket == 192000 ? 2 : (bucket == 96000 ? 1 : 0);
+	if (bucket != sr) { // "sample rate ...K upsampled to ...K." (Model.cpp:58-59)
+		h->pre = 1;
+		h->in_fmt = AISGPU_FMT_CF32;
+		h->us_inc = (float)sr / (float)bucket; // Upsample::setParams (DSP.h:172-176)
+		h->us_ratio = (bucket + sr - 1) / sr;
+		h->PA = 4;
+	}
+	h->use_fdc = (h->cfg.droop && h->k > 0) ? 1 : 0;
+	h->fdc_alpha = h->k == 2 ? -1.1f : -0.8f;
+	h->fdc_beta = 1 - 2 * h->fdc_alpha; // DSP.h:293-297
+	// history in input samples: FCIC5 5 + FDC 2 at 48 kHz, h_l = 2 h_{l-1} + 5 per CIC stage, rounded up to whole lane chunks
+	int hk = 7;
+	for (int i = 0; i < h->k; i++) hk = 2 * hk + 5;
+	const int g = frontend_x_granule(h->in_fmt);
+	h->P = (hk + g - 1) / g * g;
+	h->P96 = 0;
+	return 0;
+}
+
 // Model.cpp:129-338: which bucket, how many CIC stages, droop taps, resampler.  Returns <0 when unsupported.
 int plan_frontend(aisgpu_handle *h) {
 	const int sr = h->cfg.sample_rate;
+	if (h->cfg.channel_mode != AISGPU_MODE_AB && h->cfg.channel_mode != AISGPU_MODE_X) {
+		h->err = "unknown channel_mode (AISGPU_MODE_AB or AISGPU_MODE_X)";
+		return AISGPU_EINVAL;
+	}
+	h->xmode = h->cfg.channel_mode == AISGPU_MODE_X;
+	if (h->xmode) return plan_frontend_x(h);
 	if (sr < 96000 || sr > 12288000) {
 		h->err = "Model: sample rate must be between 96K and 12288K (inclusive).";
 		return AISGPU_EINVAL;
@@ -343,6 +393,7 @@ int plan_frontend(aisgpu_handle *h) {
 
 // granule of the caller's submit length: every CIC stage needs an even block (DSP.cpp:94,135)
 int outer_granule(const aisgpu_handle *h) {
+	if (h->xmode) return X_GRANULE;
 	if (h->fp_ds) return 16384; // 32 lane sub-segments of 512 samples: the shortest the streaming kernel takes (sub-segment >= warm-up history, 384)
 	return h->pre >= 2 ? std::max(64, 1 << (h->kA + 2)) : (1 << (h->k + h->kA + 2));
 }
@@ -368,7 +419,30 @@ void layout_frontend(FeParams &p, int k, int tile) {
 	p.tile = tile;
 }
 
+// single-channel mode: K x Downsample2CIC5 -> [FDC] -> FilterCIC5 into Cbuf row `stream` (fe_x.cu)
+int launch_frontend_single(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
+	FeParams &p = h->fe;
+	p.in = dev_in;
+	p.tail = h->d_tail[h->tail_cur];
+	p.in_stride = stride;
+	p.format = h->in_fmt;
+	p.k = h->k;
+	p.N = N;
+	p.P = h->P;
+	p.use_fdc = h->use_fdc;
+	p.fdc_alpha = h->fdc_alpha;
+	p.fdc_beta = h->fdc_beta;
+	p.rot = nullptr;
+	p.C = h->d_C2[h->chunk % aisgpu_handle::NC];
+	p.c_stride = h->c_stride;
+	p.c_off = HC;
+	p.st_B = h->cfg.n_streams;
+	CU(launch_frontend_x(p, h->in_fmt, h->k, h->st_L, h->fe_stream));
+	return 0;
+}
+
 int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
+	if (h->xmode) return launch_frontend_single(h, dev_in, stride, N);
 	FeParams &p = h->fe;
 	const int q = 1 << (h->k + 2);
 	// per-CTA tile: one run of 5 outputs per thread at the first CIC stage (2 x 5 x threads input samples)
@@ -566,6 +640,7 @@ int run_symbols(aisgpu_handle *h, int n_new) {
 			p.nslots_fm = f.nslots;
 			p.lvl_prev = h->d_lvl_prev + (size_t)h->lvlp_cur * h->rows;
 			p.lvl_prev_out = h->d_lvl_prev + (size_t)(h->lvlp_cur ^ 1) * h->rows;
+			p.lvl_own = h->xmode;
 			h->lvlp_cur ^= 1;
 			p.abs_lo = a0;
 			p.abs_hi = a1;
@@ -612,7 +687,7 @@ int enqueue_rot_table(aisgpu_handle *h, long long c, int n96) {
 
 // One Receive() of the front end proper: N samples per stream (a whole reference block) -> frames.
 int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
-	const int q = 1 << (h->k + 2);
+	const int q = h->xmode ? X_GRANULE : 1 << (h->k + 2);
 	if (N <= 0 || N > h->inner_max || (N % q) != 0) {
 		char b[160];
 		snprintf(b, sizeof(b), "internal: block of %d samples must be a positive multiple of %d and <= %d", N, q, h->inner_max);
@@ -620,9 +695,9 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 		return AISGPU_ECUDA; // cannot come from the caller's arguments (check_outer has passed): poisons the handle
 	}
 	const int k = h->k, B = h->cfg.n_streams;
-	const int n96 = N >> k, n48 = n96 >> 1;
-	// ---- K0: Rotate phasor table (side stream; normally already enqueued by the previous submit) ----
-	{
+	const int n96 = N >> k, n48 = h->xmode ? n96 : n96 >> 1; // X: the k CIC stages end at 48 kHz
+	// ---- K0: Rotate phasor table (side stream; normally already enqueued by the previous submit); single-channel mode has none ----
+	if (!h->xmode) {
 		const long long c = h->chunk;
 		const int slot = (int)(c % 3);
 		if (!(h->rot_ready_chunk == c && h->rot_n96[slot] == n96)) {
@@ -643,9 +718,12 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 	CU(cudaEventRecord(h->ev_k1[h->chunk % 3], h->fe_stream));
 	h->k1_recorded[h->chunk % 3] = true;
 	h->fe_timed = true;
-	h->last_launches += 2; // front end + this submit's phasor table
-	// speculate that the next submit has the same length: build its phasor table now, off the critical path
-	if (int rc = enqueue_rot_table(h, h->chunk + 1, n96)) return rc;
+	if (h->xmode) h->last_launches++;
+	else {
+		h->last_launches += 2; // front end + this submit's phasor table
+		// speculate that the next submit has the same length: build its phasor table now, off the critical path
+		if (int rc = enqueue_rot_table(h, h->chunk + 1, n96)) return rc;
+	}
 	// ---- front-end history for the next submit ----
 	{
 		const int nxt = h->tail_cur ^ 1;
@@ -829,7 +907,7 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 				h->outer_N = N;
 				h->us_blk = L;
 				if (h->pre == 1) h->blk = L;
-				h->s_cap = 4 * L;
+				h->s_cap = (h->us_ratio + 2) * L; // whole blocks: < L left over + up to us_ratio * L (+ a few) new samples
 			}
 			FeParams &pp = h->fe_pre;
 			int tile = 1280;
@@ -1101,8 +1179,8 @@ int drain_ring(aisgpu_handle *h, long long upto) {
 		h->counters[0]++;
 		aisgpu_msg m;
 		memset(&m, 0, sizeof(m));
-		m.stream = r.row >> 1;
-		m.channel = (r.row & 1) ? h->cfg.channel_b : h->cfg.channel_a;
+		m.stream = stream_of_row(h, r.row);
+		m.channel = channel_of_row(h, r.row) ? h->cfg.channel_b : h->cfg.channel_a;
 		m.nbits = (r.nbits >= 0 && r.nbits <= 1064) ? r.nbits : 0; // Message::setLength (Message.h:288-292)
 		m.start_idx = r.start_idx;
 		m.end_idx = r.end_idx;
@@ -1115,7 +1193,7 @@ int drain_ring(aisgpu_handle *h, long long upto) {
 		if (!msg_validate(m.data, m.nbits)) continue; // AIS.cpp:87-93: dropped, siblings were still reset
 		build_nmea(m, h->cfg.own_mmsi, &h->seq[m.stream]);
 		h->counters[1]++;
-		h->counters[(r.row & 1) ? 6 : 5]++;
+		h->counters[channel_of_row(h, r.row) ? 6 : 5]++;
 		h->out_queue.push_back(m);
 	}
 	return 0;
@@ -1151,6 +1229,7 @@ void aisgpu_default_config(aisgpu_config *cfg) {
 	cfg->fp_ds = 0;
 	cfg->dd_train = 0.75f;
 	cfg->dd_weight = 0.86f;
+	cfg->channel_mode = AISGPU_MODE_AB;
 }
 
 const char *aisgpu_last_error(aisgpu_handle *h) { return h ? h->err.c_str() : g_create_error.c_str(); }
@@ -1256,11 +1335,11 @@ static int create_impl(aisgpu_handle *h) {
 	const int q = outer_granule(h);
 	const int maxN = (c.max_chunk_samples + q - 1) / q * q;
 	h->cfg.max_chunk_samples = maxN;
-	h->rows = 2 * B;
+	h->rows = rows_of(h);
 	h->obps = bytes_per_sample(c.format);
 	h->bps = bytes_per_sample(h->in_fmt);
 	h->inner_max = h->pre == 1 ? (maxN >> h->kA) : (h->pre >= 2 ? h->blk : maxN);
-	h->max_n48 = h->inner_max >> (k + 1);
+	h->max_n48 = h->inner_max >> (h->xmode ? k : k + 1);
 	h->seq.assign(B, 0);
 	if (h->pre) { // resampler pre-stage: raw-format history, decimated stream, schedule tables, ring of reference blocks
 		const int tl = h->pre == 2 ? 32 : h->PA;
@@ -1274,9 +1353,9 @@ static int create_impl(aisgpu_handle *h) {
 			if (int rc = dalloc(h, &h->d_D0, (size_t)B * h->d0_stride)) return rc;
 			memset(&h->fe_pre, 0, sizeof(h->fe_pre));
 			if (h->pre != 4) {
-				if (int rc = dalloc(h, &h->d_us_src, (size_t)2 * Lmax + 8)) return rc;
-				if (int rc = dalloc(h, &h->d_us_alpha, (size_t)2 * Lmax + 8)) return rc;
-				h->s_stride = 4LL * Lmax;
+				if (int rc = dalloc(h, &h->d_us_src, (size_t)h->us_ratio * Lmax + 8)) return rc;
+				if (int rc = dalloc(h, &h->d_us_alpha, (size_t)h->us_ratio * Lmax + 8)) return rc;
+				h->s_stride = (long long)(h->us_ratio + 2) * Lmax;
 			}
 		}
 		if (h->pre >= 2) {
@@ -1303,10 +1382,10 @@ static int create_impl(aisgpu_handle *h) {
 			CU(cudaMemsetAsync(h->d_tail[i], 0x80, (size_t)B * h->P * h->bps, h->stream));
 		if (int rc = dalloc(h, &h->d_fir_hist[i], (size_t)h->rows * 16)) return rc;
 	}
-	for (int i = 0; i < 3; i++)
-		if (int rc = dalloc(h, &h->d_rot[i], (size_t)h->P96 + (h->inner_max >> k) + 8)) return rc;
-	if (int rc = dalloc(h, &h->d_rot_state, 4)) return rc;
-	{
+	if (!h->xmode) {
+		for (int i = 0; i < 3; i++)
+			if (int rc = dalloc(h, &h->d_rot[i], (size_t)h->P96 + (h->inner_max >> k) + 8)) return rc;
+		if (int rc = dalloc(h, &h->d_rot_state, 4)) return rc;
 		float2 one = make_float2(1.0f, 0.0f);
 		CU(cudaMemcpyAsync(h->d_rot_state, &one, sizeof(one), cudaMemcpyHostToDevice, h->stream)); // after the memset on the same stream
 		h->mult = polar1((float)(PI_F * 25000.0 / 48000.0)); // Model.cpp:31
@@ -1442,7 +1521,7 @@ static int create_impl(aisgpu_handle *h) {
 	for (int i = 0; i < aisgpu_handle::NT; i++) CU(cudaEventCreateWithFlags(&h->ev_ticket[i], cudaEventDisableTiming));
 	CU(cudaEventCreateWithFlags(&h->ev_mark, cudaEventDisableTiming));
 	if (h->pre == 1 || h->pre == 3) {
-		h->us_cap = 2 * (maxN >> h->kA) + 8; // Upsample never more than doubles the rate (bucket / 2 < rate)
+		h->us_cap = h->us_ratio * (maxN >> h->kA) + 8; // Upsample emits at most ceil(bucket / rate) samples per input
 		for (int i = 0; i < 2; i++) {
 			if (cudaMallocHost((void **)&h->pin_us_src[i], (size_t)h->us_cap * sizeof(int)) != cudaSuccess ||
 				cudaMallocHost((void **)&h->pin_us_alpha[i], (size_t)h->us_cap * sizeof(float)) != cudaSuccess) {
@@ -1461,13 +1540,24 @@ static int create_impl(aisgpu_handle *h) {
 	return 0;
 }
 
+// The caller's config: the current layout, or the one before channel_mode was appended (then AB).
+static bool copy_config(const aisgpu_config *cfg, aisgpu_config *c) {
+	if (!cfg || (cfg->struct_size != sizeof(aisgpu_config) && cfg->struct_size != offsetof(aisgpu_config, channel_mode))) return false;
+	memset(c, 0, sizeof(*c));
+	memcpy(c, cfg, cfg->struct_size);
+	c->struct_size = sizeof(aisgpu_config);
+	if (cfg->struct_size != sizeof(aisgpu_config)) c->channel_mode = AISGPU_MODE_AB;
+	return true;
+}
+
 int aisgpu_create(const aisgpu_config *cfg, aisgpu_handle **out) {
-	if (!cfg || !out || cfg->struct_size != sizeof(aisgpu_config)) {
+	aisgpu_config c;
+	if (!out || !copy_config(cfg, &c)) {
 		g_create_error = "aisgpu_create: null argument or struct_size mismatch";
 		return AISGPU_EINVAL;
 	}
 	aisgpu_handle *h = new aisgpu_handle();
-	h->cfg = *cfg;
+	h->cfg = c;
 	int rc = create_impl(h);
 	if (rc) {
 		g_create_error = h->err;
@@ -1496,6 +1586,10 @@ int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stri
 	if (!dev_samples) return AISGPU_EINVAL;
 	if (stride_samples < n_samples || (stride_samples & 1)) {
 		h->err = "stride_samples must be even and >= n_samples";
+		return AISGPU_EINVAL;
+	}
+	if (h->xmode && (((size_t)dev_samples % 16) != 0 || ((stride_samples * h->obps) % 16) != 0)) {
+		h->err = "single-channel mode: the rows of a device batch must be 16-byte aligned";
 		return AISGPU_EINVAL;
 	}
 	if (int rc = check_outer(h, n_samples)) return rc; // all argument checks come before any state is touched
@@ -1589,7 +1683,11 @@ int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, si
 	CU(cudaSetDevice(h->cfg.device));
 	CU(cudaStreamSynchronize(h->fe_stream));
 	if (int rc = sync_backend(h)) return rc;
-	const int row = stream * 2 + (channel & 1);
+	if (h->xmode && (tap == AISGPU_TAP_ROT || (channel & 1))) {
+		h->err = "single-channel mode has no Rotate and no channel 1";
+		return AISGPU_EINVAL;
+	}
+	const int row = row_of(h, stream, channel & 1);
 	const void *src = nullptr;
 	size_t n = 0, esz = 8;
 	switch (tap) {
@@ -1812,12 +1910,13 @@ int aisgpu_frontend_times(aisgpu_handle *h, float *ms_out, int max, int *n) {
 int aisgpu_last_launches(aisgpu_handle *h) { return h ? h->last_launches : 0; }
 
 int aisgpu_chunk_granule(const aisgpu_config *cfg) {
-	if (!cfg || cfg->struct_size != sizeof(aisgpu_config)) {
+	aisgpu_config c;
+	if (!copy_config(cfg, &c)) {
 		g_create_error = "aisgpu_chunk_granule: null argument or struct_size mismatch";
 		return AISGPU_EINVAL;
 	}
 	aisgpu_handle tmp;
-	tmp.cfg = *cfg;
+	tmp.cfg = c;
 	if (int rc = plan_frontend(&tmp)) {
 		g_create_error = tmp.err;
 		return rc;

@@ -1,6 +1,6 @@
 // params.h -- parameter blocks, per-row state records and launch entry points of the kernels (host and device view).
 //
-// Layout in HBM (one engine == one batch of B independent IQ streams, "row" = stream*2 + channel):
+// Layout in HBM (one engine == one batch of B independent IQ streams, "row" = stream*2 + channel; single-channel mode: row = stream):
 //   in     [B][N]              input samples of one submit (CF32 float2, or CU8/CS8/CS16)
 //   tail   [B][P]              last P input samples of the previous submit (front-end warm-up history)
 //   rot    [P96 + N>>k]        Rotate phasor table of the submit (shared by all streams), with P96 history
@@ -117,6 +117,7 @@ struct K3Params {
 	int nslots_fm;        // ModelChallenger: slots the FM branch covers this submit
 	const float *lvl_prev; // ModelChallenger: [rows] the level the tag carries into this block (read)
 	float *lvl_prev_out;   //                  ... and into the next one (written; double buffered by launch)
+	int lvl_own;           //                  1 (single-channel mode): a row carries its own last level; 0: channel A the one B left
 	int dwords;
 	float *lvl;           // ModelDefault: ScatterPLL level of symbol s (TAG::sample_lvl, DSP.h:100-106), [rows][lvl_stride]
 	int lvl_stride;
@@ -184,6 +185,9 @@ cudaError_t launch_frontend_stream(const FeParams &p, int fmt, int k, bool pre, 
 cudaError_t launch_frontend_stream_fpds(const FeParams &p, int forced_L, cudaStream_t s); // fe_stream_fp.cu: CU8, integer CIC stages, 1536K
 template <int FMT, int G, int NB, int WPC>
 cudaError_t launch_frontend_stream_shape(const FeParams &p, int k, bool pre, int forced_L, cudaStream_t s);
+// fe_x.cu: single-channel mode, k = 0 .. 2 CIC stages, one Cbuf row per stream; p.N and p.P multiples of frontend_x_granule(fmt)
+cudaError_t launch_frontend_x(const FeParams &p, int fmt, int k, int forced_L, cudaStream_t s);
+int frontend_x_granule(int fmt);
 // be_cgf.cu
 cudaError_t cgf_init(const float *taps17, const float2 *omega256);
 cudaError_t launch_cgf_estimate(const float2 *Cbuf, long long c_stride, int c_begin, int nblk, int total_blocks, const float2 *omega, int wide, int *stepidx, cudaStream_t s);

@@ -110,7 +110,11 @@ public:
 	void buildModel(char CH1, char CH2, int sample_rate, bool timerOn, Device::Device *dev) override {
 		device = dev;
 		if (!device) throw std::runtime_error("ModelGPU: no device");
-		if (mode != Mode::AB) throw std::runtime_error("ModelGPU: only two-channel (AB/CD) mode is built");
+		// AB and CD build the same chain (only the letters and the tuning differ, Receiver.cpp:81-86); X is the single-channel chain
+		// (Model.cpp:35-107), whose frames carry CH1
+		if (mode == Mode::AB || mode == Mode::CD) cfg.channel_mode = AISGPU_MODE_AB;
+		else if (mode == Mode::X) cfg.channel_mode = AISGPU_MODE_X;
+		else throw std::runtime_error("ModelGPU: only the AB, CD and X channel modes are built");
 		cfg.sample_rate = sample_rate;
 		cfg.channel_a = CH1;
 		cfg.channel_b = CH2;

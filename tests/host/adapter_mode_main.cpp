@@ -1,0 +1,86 @@
+// Test program for ais-catcher_b200/host/ModelGPU.h in a channel mode other than AB: the adapter inside the reference's own
+// block graph, with Model::setMode called before buildModel as the Receiver does (Source/Application/Receiver.cpp:81-98).
+//
+//   adapter_mode_test <X|CD> <file> <format CU8|CF32> <sample_rate> <block_samples> [cpu]
+//
+// Wires MemDevice --Connection<RAW>--> AIS::ModelGPU(ModelDefault kind) --StreamOut<Message>--> sink, or the reference's own
+// ModelDefault with the trailing "cpu" (an A/B in one binary), with the Receiver's default letters of the mode ("XX" / 'C','D').
+// Prints one line per message: channel|nbits|start|end|level-bits|ppm-bits|sentence[ sentence...]
+// Exit code 3 = the adapter reported a run-time failure through Error() + StopRequest(); 4 = configuration error.
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <string>
+#include <vector>
+
+#include "Device.h"
+#include "Model.h"
+#include "ModelGPU.h"
+
+static int g_stop_requests = 0;
+void StopRequest() { g_stop_requests++; } // Source/Library/Common.h:72 -- the application normally defines it
+
+namespace {
+struct MemDevice : public Device::Device {
+	void push(void *p, int bytes, Format f) {
+		RAW r{f, p, bytes};
+		Send(&r, 1, tag);
+	}
+};
+struct Sink : public StreamIn<AIS::Message> {
+	long count = 0;
+	void Receive(const AIS::Message *m, int len, TAG &tag) override {
+		for (int i = 0; i < len; i++) {
+			unsigned lb, pb;
+			memcpy(&lb, &tag.level, 4);
+			memcpy(&pb, &tag.ppm, 4);
+			printf("%c|%d|%lld|%lld|%u|%u|", m[i].getChannel(), m[i].getLength(), (long long)m[i].start_idx, (long long)m[i].end_idx, lb, pb);
+			bool first = true;
+			for (const auto &s : m[i].sentences()) {
+				if (!first) putchar(' ');
+				fwrite(s.data(), 1, s.size(), stdout);
+				first = false;
+			}
+			putchar('\n');
+			count++;
+		}
+	}
+};
+} // namespace
+
+int main(int argc, char **argv) {
+	if (argc < 6) {
+		fprintf(stderr, "usage: %s X|CD file CU8|CF32 rate block_samples [cpu]\n", argv[0]);
+		return 2;
+	}
+	const bool x = strcmp(argv[1], "X") == 0;
+	const Format fmt = strcmp(argv[3], "CF32") == 0 ? Format::CF32 : Format::CU8;
+	const int bps = fmt == Format::CF32 ? 8 : 2;
+	const int rate = atoi(argv[4]), block = atoi(argv[5]);
+	const bool cpu = argc > 6 && strcmp(argv[6], "cpu") == 0;
+	FILE *f = fopen(argv[2], "rb");
+	if (!f) { perror(argv[2]); return 2; }
+	std::vector<unsigned char> data;
+	unsigned char buf[65536];
+	size_t n;
+	while ((n = fread(buf, 1, sizeof(buf), f)) > 0) data.insert(data.end(), buf, buf + n);
+	fclose(f);
+
+	MemDevice dev;
+	Sink sink;
+	AIS::Model *model = cpu ? (AIS::Model *)new AIS::ModelDefault() : (AIS::Model *)new AIS::ModelGPU(AISGPU_MODEL_DEFAULT);
+	try {
+		model->setMode(x ? AIS::Mode::X : AIS::Mode::CD);
+		model->buildModel(x ? 'X' : 'C', x ? 'X' : 'D', rate, false, &dev);
+	}
+	catch (std::exception &e) {
+		fprintf(stderr, "config error: %s\n", e.what());
+		return 4;
+	}
+	model->Output().out.Connect(&sink);
+	const size_t step = (size_t)block * bps;
+	for (size_t off = 0; off + step <= data.size() && !g_stop_requests; off += step) dev.push(data.data() + off, (int)step, fmt);
+	fprintf(stderr, "%ld messages, %d stop requests\n", sink.count, g_stop_requests);
+	delete model;
+	return g_stop_requests ? 3 : 0;
+}

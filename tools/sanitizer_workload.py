@@ -5,6 +5,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "ais-catcher_b200")); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
 import aisgpu, aissynth
+sys.path.insert(0, os.path.join(ROOT, "oracle"))
+import mode_x_util
 import __graft_entry__ as g
 
 g.smoke()
@@ -33,6 +35,17 @@ for c in range(3):
     eng.submit(np.ascontiguousarray(x6[:, c * 32768:(c + 1) * 32768]), 32768)
 print("6 MSPS messages", len(eng.poll()))
 eng.close()
+for fs_x, fmt, model in ((192000, aisgpu.FMT_CS16, aisgpu.MODEL_CHALLENGER), (12000, aisgpu.FMT_CF32, aisgpu.MODEL_DEFAULT)):  # single-channel mode, odd batch
+    nx = 64 * 37
+    xx = [mode_x_util.x_stream(fs_x, nx * 3, 500 + s)[0] for s in range(3)]
+    eng = aisgpu.Engine(model=model, sample_rate=fs_x, fmt=fmt, n_streams=3, max_chunk=nx, channel_mode=aisgpu.MODE_X)
+    for c in range(3):
+        blk = [x[c * nx:(c + 1) * nx] for x in xx]
+        if fmt == aisgpu.FMT_CS16:
+            blk = [np.clip(np.round(np.stack([b.real, b.imag], 1).ravel() * 32767.0), -32768, 32767).astype(np.int16) for b in blk]
+        eng.submit(np.stack(blk), nx)
+    print("X mode", fs_x, "messages", len(eng.poll()))
+    eng.close()
 with tempfile.TemporaryDirectory() as d:  # file feeder, CU8, ragged lengths, FP_DS integer front end
     paths = []
     for s in range(2):
