@@ -11,6 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("AISGPU_LIB") or os.path.join(HERE, "libaisgpu.so")  # AISGPU_LIB: A/B of two builds of the library on one machine
 
 MODEL_STANDARD, MODEL_BASE, MODEL_DEFAULT, MODEL_CHALLENGER, MODEL_V2 = 0, 1, 2, 4, 11
+MODEL_DISCRIMINATOR = 3  # FM-discriminator input: I and Q are the audio of two discriminator taps (channels A and B)
 FMT_CF32, FMT_CU8, FMT_CS8, FMT_CS16 = 0, 1, 2, 3
 MODE_AB, MODE_X = 0, 3  # aisgpu_config.channel_mode: two channels (also CD) / single channel (-c X)
 TAP_C, TAP_CGF, TAP_FIR, TAP_ROT, TAP_DEC, TAP_FM, TAP_PRE, TAP_PRE2 = 0, 1, 2, 3, 4, 5, 7, 8

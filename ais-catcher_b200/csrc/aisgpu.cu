@@ -62,7 +62,8 @@ constexpr int V2_BLK = 512; // V2::BLOCK_SIZE (V2Engine.h:30)
 constexpr int HD = 48;  // ModelChallenger: derotated samples kept in front of the new ones (FM needs 1, FIR37 36, a partial group 4)
 constexpr int HE = 8;   // room in front of new symbol-stage samples: an incomplete group of 5 (<=4)
 
-constexpr int X_GRANULE = 64; // single-channel mode: a multiple of every format's front-end lane chunk (frontend_x_granule)
+constexpr int X_GRANULE = 64; // single-channel mode: a multiple of every format's front-end lane chunk (frontend_x_granule); also the
+                              // FM-discriminator input model's granule
 
 int bytes_per_sample(int fmt) { return fmt == AISGPU_FMT_CF32 ? 8 : (fmt == AISGPU_FMT_CS16 ? 4 : 2); }
 
@@ -101,6 +102,7 @@ struct aisgpu_handle {
 	int use_fdc = 0;
 	int fp_ds = 0; // integer CIC front end (DS_UINT16 x 4, DSP.cpp:499-665): CU8 @1536K with -go FP_DS on
 	int xmode = 0; // single-channel mode (AISGPU_MODE_X): no Rotate, one back-end row per stream
+	int disc = 0;  // FM-discriminator input (AISGPU_MODEL_DISCRIMINATOR): I and Q are two real 48 kHz rows, no Rotate, no CIC stage
 	int us_ratio = 2; // ceil(bucket / rate): most DSP::Upsample outputs per input sample (AB: <= 2, X: <= 4)
 	float fdc_alpha = 0, fdc_beta = 1;
 	int rows = 0;
@@ -299,6 +301,37 @@ int plan_frontend_x(aisgpu_handle *h) {
 	return 0;
 }
 
+// Model.cpp:702-731 (-m 3): convert at 48 kHz, Upsample(fs -> 48000) straight behind convert below it, never a CIC stage; the
+// channel mode is not read (ModelDiscriminator is a Model, not a ModelFrontend), and neither are droop / DSK / FP_DS.
+int plan_frontend_disc(aisgpu_handle *h) {
+	const int sr = h->cfg.sample_rate;
+	if (sr > 48000) {
+		h->err = "Internal error: sample rate not supported in FM discriminator model.";
+		return AISGPU_EINVAL;
+	}
+	if (sr < 12000) { // the reference takes any lower rate; the Upsample ring here holds ratios up to 4 (< 1.25 samples per symbol below)
+		h->err = "FM discriminator model: sample rate must be between 12k and 48k (inclusive).";
+		return AISGPU_EINVAL;
+	}
+	h->disc = 1;
+	h->pre = 0;
+	h->kA = 0;
+	h->k = 0;
+	h->fp_ds = 0;
+	h->in_fmt = h->cfg.format;
+	if (sr != 48000) { // US.setParams(sample_rate, 48000) (Model.cpp:722-728)
+		h->pre = 1;
+		h->in_fmt = AISGPU_FMT_CF32;
+		h->us_inc = (float)sr / 48000.0f; // Upsample::setParams (DSP.h:172-176)
+		h->us_ratio = (48000 + sr - 1) / sr;
+		h->PA = 4;
+	}
+	h->use_fdc = 0;
+	h->P = 0; // the split has no filter state: no warm-up history
+	h->P96 = 0;
+	return 0;
+}
+
 // Model.cpp:129-338: which bucket, how many CIC stages, droop taps, resampler.  Returns <0 when unsupported.
 int plan_frontend(aisgpu_handle *h) {
 	const int sr = h->cfg.sample_rate;
@@ -306,6 +339,7 @@ int plan_frontend(aisgpu_handle *h) {
 		h->err = "unknown channel_mode (AISGPU_MODE_AB or AISGPU_MODE_X)";
 		return AISGPU_EINVAL;
 	}
+	if (h->cfg.model == AISGPU_MODEL_DISCRIMINATOR) return plan_frontend_disc(h); // the same two-row chain in AB and X
 	h->xmode = h->cfg.channel_mode == AISGPU_MODE_X;
 	if (h->xmode) return plan_frontend_x(h);
 	if (sr < 96000 || sr > 12288000) {
@@ -393,7 +427,7 @@ int plan_frontend(aisgpu_handle *h) {
 
 // granule of the caller's submit length: every CIC stage needs an even block (DSP.cpp:94,135)
 int outer_granule(const aisgpu_handle *h) {
-	if (h->xmode) return X_GRANULE;
+	if (h->xmode || h->disc) return X_GRANULE;
 	if (h->fp_ds) return 16384; // 32 lane sub-segments of 512 samples: the shortest the streaming kernel takes (sub-segment >= warm-up history, 384)
 	return h->pre >= 2 ? std::max(64, 1 << (h->kA + 2)) : (1 << (h->k + h->kA + 2));
 }
@@ -441,8 +475,24 @@ int launch_frontend_single(aisgpu_handle *h, const void *dev_in, long long strid
 	return 0;
 }
 
+// FM-discriminator input: ConvertRAW, I into Cbuf row 2 * stream and Q into row 2 * stream + 1 as real samples (fe_disc.cu)
+int launch_frontend_split(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
+	FeParams &p = h->fe;
+	p.in = dev_in;
+	p.in_stride = stride;
+	p.format = h->in_fmt;
+	p.N = N;
+	p.C = h->d_C2[h->chunk % aisgpu_handle::NC];
+	p.c_stride = h->c_stride;
+	p.c_off = HC;
+	p.st_B = h->cfg.n_streams;
+	CU(launch_frontend_disc(p, h->in_fmt, h->fe_stream));
+	return 0;
+}
+
 int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	if (h->xmode) return launch_frontend_single(h, dev_in, stride, N);
+	if (h->disc) return launch_frontend_split(h, dev_in, stride, N);
 	FeParams &p = h->fe;
 	const int q = 1 << (h->k + 2);
 	// per-CTA tile: one run of 5 outputs per thread at the first CIC stage (2 x 5 x threads input samples)
@@ -526,12 +576,16 @@ int carry2(aisgpu_handle *h, const float2 *src, float2 *dst, long long stride, i
 	return 0;
 }
 
+// ModelStandard's tail, Filter 37 -> Deinterleave(5) -> 5 cross-reset decoders (Model.cpp:484-518), which ModelDiscriminator
+// repeats behind its real rows (Model.cpp:732-751)
+bool standard_tail(const aisgpu_handle *h) { return h->cfg.model == AISGPU_MODEL_STANDARD || h->cfg.model == AISGPU_MODEL_DISCRIMINATOR; }
+
 int run_symbols(aisgpu_handle *h, int n_new) {
 	// n_new samples were appended at [HE, HE + n_new) of every row of Ec/Ef.
 	// ModelDefault (ScatterPLL, DSP.h:95-117) only forwards complete groups of 5: e_left older samples sit just
 	// before HE and the incomplete group at the end is carried.  ModelStandard (Deinterleave, DSP.h:65-73)
 	// forwards every sample at once, so partial groups at both ends are walked with a per-phase validity test.
-	if (h->cfg.model == AISGPU_MODEL_STANDARD) {
+	if (standard_tail(h)) {
 		const long long a0 = h->e_abs, a1 = a0 + n_new;
 		const long long g0 = a0 - a0 % 5;
 		const int nslots = (int)((a1 - g0 + 4) / 5);
@@ -687,7 +741,7 @@ int enqueue_rot_table(aisgpu_handle *h, long long c, int n96) {
 
 // One Receive() of the front end proper: N samples per stream (a whole reference block) -> frames.
 int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
-	const int q = h->xmode ? X_GRANULE : 1 << (h->k + 2);
+	const int q = (h->xmode || h->disc) ? X_GRANULE : 1 << (h->k + 2);
 	if (N <= 0 || N > h->inner_max || (N % q) != 0) {
 		char b[160];
 		snprintf(b, sizeof(b), "internal: block of %d samples must be a positive multiple of %d and <= %d", N, q, h->inner_max);
@@ -695,9 +749,10 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 		return AISGPU_ECUDA; // cannot come from the caller's arguments (check_outer has passed): poisons the handle
 	}
 	const int k = h->k, B = h->cfg.n_streams;
-	const int n96 = N >> k, n48 = h->xmode ? n96 : n96 >> 1; // X: the k CIC stages end at 48 kHz
-	// ---- K0: Rotate phasor table (side stream; normally already enqueued by the previous submit); single-channel mode has none ----
-	if (!h->xmode) {
+	const int n96 = N >> k, n48 = (h->xmode || h->disc) ? n96 : n96 >> 1; // X: the k CIC stages end at 48 kHz; -m 3: no CIC stage
+	// ---- K0: Rotate phasor table (side stream; normally already enqueued by the previous submit); single-channel mode and the
+	// FM-discriminator input have none ----
+	if (!h->xmode && !h->disc) {
 		const long long c = h->chunk;
 		const int slot = (int)(c % 3);
 		if (!(h->rot_ready_chunk == c && h->rot_n96[slot] == n96)) {
@@ -718,14 +773,14 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 	CU(cudaEventRecord(h->ev_k1[h->chunk % 3], h->fe_stream));
 	h->k1_recorded[h->chunk % 3] = true;
 	h->fe_timed = true;
-	if (h->xmode) h->last_launches++;
+	if (h->xmode || h->disc) h->last_launches++;
 	else {
 		h->last_launches += 2; // front end + this submit's phasor table
 		// speculate that the next submit has the same length: build its phasor table now, off the critical path
 		if (int rc = enqueue_rot_table(h, h->chunk + 1, n96)) return rc;
 	}
-	// ---- front-end history for the next submit ----
-	{
+	// ---- front-end history for the next submit (none for the FM-discriminator input's split) ----
+	if (h->P) {
 		const int nxt = h->tail_cur ^ 1;
 		const int p_w = h->P * h->bps / 8;
 		CU(launch_tail_update(h->d_tail[nxt], h->d_tail[h->tail_cur], dev_in, stride * h->bps / 8, (long long)N * h->bps / 8, p_w, B, h->fe_stream));
@@ -806,7 +861,10 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 	}
 	else {
 		if (int rc = stage_begin(h, 5)) return rc;
-		if (int rc = carry2(h, Ccur, Cnext, h->c_stride, HC + n48 - FIRF_T, HC - FIRF_T, FIRF_T)) return rc; // FM + FIR history
+		if (h->disc) { // FIR history of the real rows: the last 36 samples (n48 is even), moved as 18 float2
+			if (int rc = carry2(h, Ccur, Cnext, h->c_stride, HC + n48 / 2 - (FIRF_T - 1) / 2, HC - (FIRF_T - 1) / 2, (FIRF_T - 1) / 2)) return rc;
+		}
+		else if (int rc = carry2(h, Ccur, Cnext, h->c_stride, HC + n48 - FIRF_T, HC - FIRF_T, FIRF_T)) return rc; // FM + FIR history
 		if (int rc = stage_end(h, 5)) return rc;
 		{
 			// the 5-phase deinterleaver's slots are aligned to absolute sample indices (DSP.h:65-73)
@@ -819,7 +877,7 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 			f.c_stride = h->c_stride;
 			f.c_new = HC;
 			f.n = n48;
-			f.r0 = h->cfg.model == AISGPU_MODEL_STANDARD ? (int)(a0 - g0) : 0;
+			f.r0 = standard_tail(h) ? (int)(a0 - g0) : 0;
 			f.nslots = nslots;
 			// the filtered samples themselves are only read by k_base, the bit-serial cross-check decoder and the taps
 			f.Fbuf = (h->cfg.model == AISGPU_MODEL_BASE || h->decoder == 1 || h->cfg.enable_taps) ? h->d_Ef2[0] : nullptr;
@@ -827,9 +885,10 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 			f.f_off = HE;
 			f.dbits = h->d_dbits2[h->pb];
 			f.dwords = h->dwords;
-			f.tap_fm = h->cfg.enable_taps ? h->d_tap_fm : nullptr;
+			f.tap_fm = h->cfg.enable_taps ? h->d_tap_fm : nullptr; // not allocated for the FM-discriminator input (no FM stage)
 			f.tap_stride = h->r_stride;
-			f.tap_dec = (h->cfg.enable_taps && h->cfg.model == AISGPU_MODEL_STANDARD) ? h->d_tap_dec : nullptr;
+			f.tap_dec = (h->cfg.enable_taps && standard_tail(h)) ? h->d_tap_dec : nullptr;
+			f.real = h->disc;
 			if (int rc = stage_begin(h, 0)) return rc; // Ef (single buffered) is only read by taps / k_base, which do not pipeline
 			CU(launch_fm_fir5(f, h->rows, h->bs));
 			if (int rc = stage_end(h, 0)) return rc;
@@ -838,7 +897,7 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 		h->be_recorded[cb] = true;
 		h->last_launches++;
 		h->last_nE = n48;
-		if (h->cfg.model == AISGPU_MODEL_STANDARD) {
+		if (standard_tail(h)) {
 			if (int rc = run_symbols(h, n48)) return rc;
 		}
 		else {
@@ -1241,7 +1300,7 @@ void aisgpu_internal_set_error(aisgpu_handle *h, const char *msg) { h->err = msg
 static int create_impl(aisgpu_handle *h) {
 	const aisgpu_config &c = h->cfg;
 	if (c.model != AISGPU_MODEL_DEFAULT && c.model != AISGPU_MODEL_STANDARD && c.model != AISGPU_MODEL_BASE && c.model != AISGPU_MODEL_V2 &&
-		c.model != AISGPU_MODEL_CHALLENGER) {
+		c.model != AISGPU_MODEL_CHALLENGER && c.model != AISGPU_MODEL_DISCRIMINATOR) {
 		h->err = "unknown model kind";
 		return AISGPU_EINVAL;
 	}
@@ -1258,7 +1317,7 @@ static int create_impl(aisgpu_handle *h) {
 #endif
 	// rows per warp of the decoder kernel, chosen per chain on the previous target (not re-measured on the H100): the coherent
 	// chain 1; the FM chain 3 with the current front-end shape (slightly faster than 6 rows per warp)
-	h->dec_rpw = c.model == AISGPU_MODEL_DEFAULT ? 1 : (c.model == AISGPU_MODEL_STANDARD ? 3 : 6);
+	h->dec_rpw = c.model == AISGPU_MODEL_DEFAULT ? 1 : (standard_tail(h) ? 3 : 6);
 	if (const char *e = getenv("AISGPU_DEC_RPW")) {
 		h->dec_rpw = atoi(e);
 		if (h->dec_rpw != 1 && h->dec_rpw != 3) h->dec_rpw = 6;
@@ -1303,7 +1362,7 @@ static int create_impl(aisgpu_handle *h) {
 		// target.  For the coherent chain it is what keeps the step time stable: with one back-end stream the run can lock into a serial
 		// pattern (front end c+1 starved while back end c runs, back end c+1 then waiting for it) that costs about half again per step,
 		// self-sustaining from the first submits on (tools/default_probe.py shows which pattern a process lands in).
-		const bool pipe = (e ? atoi(e) != 0 : (c.model == AISGPU_MODEL_STANDARD || c.model == AISGPU_MODEL_DEFAULT || c.model == AISGPU_MODEL_CHALLENGER)) && !c.enable_taps &&
+		const bool pipe = (e ? atoi(e) != 0 : (standard_tail(h) || c.model == AISGPU_MODEL_DEFAULT || c.model == AISGPU_MODEL_CHALLENGER)) && !c.enable_taps &&
 						  c.model != AISGPU_MODEL_BASE && c.model != AISGPU_MODEL_V2;
 		if (pipe) CU(cudaStreamCreateWithPriority(&h->be_streams[1], cudaStreamNonBlocking, prio_hi));
 	}
@@ -1339,7 +1398,7 @@ static int create_impl(aisgpu_handle *h) {
 	h->obps = bytes_per_sample(c.format);
 	h->bps = bytes_per_sample(h->in_fmt);
 	h->inner_max = h->pre == 1 ? (maxN >> h->kA) : (h->pre >= 2 ? h->blk : maxN);
-	h->max_n48 = h->inner_max >> (h->xmode ? k : k + 1);
+	h->max_n48 = h->inner_max >> ((h->xmode || h->disc) ? k : k + 1);
 	h->seq.assign(B, 0);
 	if (h->pre) { // resampler pre-stage: raw-format history, decimated stream, schedule tables, ring of reference blocks
 		const int tl = h->pre == 2 ? 32 : h->PA;
@@ -1377,12 +1436,14 @@ static int create_impl(aisgpu_handle *h) {
 		if (int rc = dalloc(h, &h->d_S, (size_t)B * h->s_stride)) return rc;
 	}
 	for (int i = 0; i < 2; i++) {
-		if (int rc = dalloc(h, &h->d_tail[i], (size_t)B * h->P * h->bps)) return rc;
-		if (h->in_fmt == AISGPU_FMT_CU8 && !h->fp_ds) // the reference's zero initial filter state is byte value 128 in CU8 (0 for the unbiased integer pipeline)
-			CU(cudaMemsetAsync(h->d_tail[i], 0x80, (size_t)B * h->P * h->bps, h->stream));
+		if (h->P) {
+			if (int rc = dalloc(h, &h->d_tail[i], (size_t)B * h->P * h->bps)) return rc;
+			if (h->in_fmt == AISGPU_FMT_CU8 && !h->fp_ds) // the reference's zero initial filter state is byte value 128 in CU8 (0 for the unbiased integer pipeline)
+				CU(cudaMemsetAsync(h->d_tail[i], 0x80, (size_t)B * h->P * h->bps, h->stream));
+		}
 		if (int rc = dalloc(h, &h->d_fir_hist[i], (size_t)h->rows * 16)) return rc;
 	}
-	if (!h->xmode) {
+	if (!h->xmode && !h->disc) {
 		for (int i = 0; i < 3; i++)
 			if (int rc = dalloc(h, &h->d_rot[i], (size_t)h->P96 + (h->inner_max >> k) + 8)) return rc;
 		if (int rc = dalloc(h, &h->d_rot_state, 4)) return rc;
@@ -1488,7 +1549,8 @@ static int create_impl(aisgpu_handle *h) {
 			CU(cudaStreamSynchronize(h->stream));
 		}
 		if (c.enable_taps) {
-			if (int rc = dalloc(h, &h->d_tap_fm, (size_t)h->rows * h->r_stride)) return rc;
+			if (!h->disc)
+				if (int rc = dalloc(h, &h->d_tap_fm, (size_t)h->rows * h->r_stride)) return rc;
 			if (int rc = dalloc(h, &h->d_tap_cnt, (size_t)h->rows)) return rc;
 		}
 	}
@@ -1687,6 +1749,10 @@ int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, si
 		h->err = "single-channel mode has no Rotate and no channel 1";
 		return AISGPU_EINVAL;
 	}
+	if (h->disc && tap == AISGPU_TAP_ROT) {
+		h->err = "the FM discriminator model has no Rotate";
+		return AISGPU_EINVAL;
+	}
 	const int row = row_of(h, stream, channel & 1);
 	const void *src = nullptr;
 	size_t n = 0, esz = 8;
@@ -1694,6 +1760,7 @@ int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, si
 	case AISGPU_TAP_C:
 		src = h->d_C2[h->c_last] + (long long)row * h->c_stride + HC; // note: valid until the next submit only for [0, n48)
 		n = h->last_n48;
+		if (h->disc) esz = 4; // real rows
 		break;
 	case AISGPU_TAP_CGF:
 		if (!h->d_tap_cgf) { h->err = "taps not enabled or not a ModelDefault engine"; return AISGPU_EINVAL; }
@@ -1731,7 +1798,7 @@ int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, si
 		else {
 			src = h->d_tap_dec + (long long)(row * 5 + phase) * h->last_nsym;
 			n = h->last_nsym;
-			if (h->cfg.model == AISGPU_MODEL_STANDARD) { // samples of this phase among the last submit's [a0, a1)
+			if (standard_tail(h)) { // samples of this phase among the last submit's [a0, a1)
 				const long long a1 = h->e_abs, a0 = a1 - h->last_nE;
 				n = 0;
 				for (long long a = a0; a < a1; a++) n += (a % 5) == phase;

@@ -10,6 +10,9 @@ __constant__ float c_taps_receiver[37];
 // 41 discriminator values are read once into registers and reused by the five 37-tap sums (each still accumulated
 // in the reference's order, k = 0..36 from 0.0f).  Besides the filtered samples the kernel emits what the decoders
 // actually consume: one sign bit per (row, sampling phase, slot), packed 32 slots per word by warp ballots.
+// REAL: the row already holds the discriminator output (ModelDiscriminator, Model.cpp:716-728: RealPart / ImaginaryPart
+// straight into Filter 37), stored as floats in the bytes of the complex row, sample m at float 2 * c_new + m.
+template <bool REAL>
 __global__ void __launch_bounds__(FM5_THREADS) k_fm_fir5(const Fm5Params p) {
 	__shared__ float fm[FM5_SAMPLES + FIRF_T - 1 + 3];
 	const int row = blockIdx.y, tid = threadIdx.x;
@@ -20,6 +23,10 @@ __global__ void __launch_bounds__(FM5_THREADS) k_fm_fir5(const Fm5Params p) {
 		const int m = M0 + i - (FIRF_T - 1);
 		float v = 0.0f;
 		if (m < p.n && m >= -(FIRF_T - 1) - 4) {
+			if (REAL) {
+				fm[i] = reinterpret_cast<const float *>(c)[m];
+				continue;
+			}
 			const float2 a = c[m], pv = c[m - 1];
 			const float re = __fsub_rn(__fmul_rn(a.x, pv.x), __fmul_rn(a.y, -pv.y));
 			const float im = __fadd_rn(__fmul_rn(a.x, -pv.y), __fmul_rn(a.y, pv.x));
@@ -58,7 +65,8 @@ __global__ void __launch_bounds__(FM5_THREADS) k_fm_fir5(const Fm5Params p) {
 cudaError_t fm_init(const float *taps37) { return cudaMemcpyToSymbol(c_taps_receiver, taps37, FIRF_T * sizeof(float)); }
 cudaError_t launch_fm_fir5(const Fm5Params &p, int rows, cudaStream_t s) {
 	dim3 grid((p.nslots + FM5_THREADS - 1) / FM5_THREADS, rows);
-	k_fm_fir5<<<grid, FM5_THREADS, 0, s>>>(p);
+	if (p.real) k_fm_fir5<true><<<grid, FM5_THREADS, 0, s>>>(p);
+	else k_fm_fir5<false><<<grid, FM5_THREADS, 0, s>>>(p);
 	return cudaGetLastError();
 }
 

@@ -4,7 +4,8 @@
 //   in     [B][N]              input samples of one submit (CF32 float2, or CU8/CS8/CS16)
 //   tail   [B][P]              last P input samples of the previous submit (front-end warm-up history)
 //   rot    [P96 + N>>k]        Rotate phasor table of the submit (shared by all streams), with P96 history
-//   Cbuf   [2B][HC + n48max]   48 kHz channel samples; new samples land at offset HC, unconsumed/history before
+//   Cbuf   [2B][HC + n48max]   48 kHz channel samples; new samples land at offset HC, unconsumed/history before (FM-discriminator
+//                              input: real samples in the same bytes, new ones from float 2 * HC)
 //   Ebuf   [2B][HE + nEmax]    samples entering the symbol-timing stage (FIR17 out, or FIR37 out for FM models)
 //   state  PS/decoder/CGF/FIR  small per-row / per-(row,phase) structs
 //   frames ring of FrameRec    decoded frames of the submit
@@ -71,6 +72,7 @@ struct Fm5Params {
 	float *tap_fm;       // optional
 	long long tap_stride;
 	float *tap_dec;      // optional: decoder input samples [rows*5][nslots], valid ones only, packed per phase
+	int real;            // 1: the rows hold real samples (the FM-discriminator input model) that go straight into FIR37
 };
 
 enum { ST_TRAINING = 0, ST_STARTFLAG = 1, ST_DATAFCS = 3 };
@@ -188,6 +190,9 @@ cudaError_t launch_frontend_stream_shape(const FeParams &p, int k, bool pre, int
 // fe_x.cu: single-channel mode, k = 0 .. 2 CIC stages, one Cbuf row per stream; p.N and p.P multiples of frontend_x_granule(fmt)
 cudaError_t launch_frontend_x(const FeParams &p, int fmt, int k, int forced_L, cudaStream_t s);
 int frontend_x_granule(int fmt);
+// fe_disc.cu: FM-discriminator input (-m 3), ConvertRAW and the I / Q split into real rows 2 * stream (I) and 2 * stream + 1 (Q) of
+// p.C, sample i at float 2 * p.c_off + i; p.N even
+cudaError_t launch_frontend_disc(const FeParams &p, int fmt, cudaStream_t s);
 // be_cgf.cu
 cudaError_t cgf_init(const float *taps17, const float2 *omega256);
 cudaError_t launch_cgf_estimate(const float2 *Cbuf, long long c_stride, int c_begin, int nblk, int total_blocks, const float2 *omega, int wide, int *stepidx, cudaStream_t s);

@@ -46,6 +46,16 @@ for fs_x, fmt, model in ((192000, aisgpu.FMT_CS16, aisgpu.MODEL_CHALLENGER), (12
         eng.submit(np.stack(blk), nx)
     print("X mode", fs_x, "messages", len(eng.poll()))
     eng.close()
+import disc_util
+for fs_d, fmt in ((48000, aisgpu.FMT_CS16), (44100, aisgpu.FMT_CF32)):  # FM-discriminator input (-m 3); 44100 through the Upsample pre-stage
+    nd = 64 * 69
+    xd = [disc_util.stream_input(fs_d, nd * 3, 600 + s, fmt)[0] for s in range(3)]
+    eng = aisgpu.Engine(model=aisgpu.MODEL_DISCRIMINATOR, sample_rate=fs_d, fmt=fmt, n_streams=3, max_chunk=nd)
+    per = 1 if fmt == aisgpu.FMT_CF32 else 2
+    for c in range(3):
+        eng.submit(np.stack([x[c * nd * per:(c + 1) * nd * per] for x in xd]), nd)
+    print("-m 3", fs_d, "messages", len(eng.poll()))
+    eng.close()
 with tempfile.TemporaryDirectory() as d:  # file feeder, CU8, ragged lengths, FP_DS integer front end
     paths = []
     for s in range(2):
