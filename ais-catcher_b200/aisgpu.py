@@ -21,7 +21,7 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_last_frontend_ms", "aisgpu_frontend_times", "aisgpu_last_launches", "aisgpu_last_error", "aisgpu_destroy",
            "aisgpu_validate", "aisgpu_build_nmea", "aisgpu_chunk_granule", "aisgpu_join", "aisgpu_submit_v", "aisgpu_submit_async",
            "aisgpu_poll_upto", "aisgpu_nccl_unique_id", "aisgpu_comm_init", "aisgpu_allreduce_counts",
-           "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files"]
+           "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW = 0, -1, -2, -3, -4, -5
 
@@ -110,6 +110,8 @@ def load():
     lib.aisgpu_last_error.argtypes = [C.c_void_p]
     lib.aisgpu_last_error.restype = C.c_char_p
     lib.aisgpu_chunk_granule.argtypes = [C.POINTER(Config)]
+    if hasattr(lib, "aisgpu_check_device_batch"):  # absent from libraries built before the placement rule (AISGPU_LIB)
+        lib.aisgpu_check_device_batch.argtypes = [C.POINTER(Config), C.c_void_p, C.c_int64]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -132,6 +134,20 @@ def chunk_granule(sample_rate, model=MODEL_DEFAULT, dsk=False, fp_ds=False, fmt=
     if g <= 0:
         raise AisGpuError("rc=%d: %s" % (g, lib.aisgpu_last_error(None).decode()))
     return g
+
+
+def check_device_batch(dev_ptr, stride_samples, sample_rate=1536000, model=MODEL_DEFAULT, fmt=FMT_CF32, dsk=False, fp_ds=False,
+                       channel_mode=MODE_AB, n_streams=1):
+    """aisgpu_check_device_batch: the placement rule of submit_device (no GPU needed).  Raises with the reason if the batch
+    may not lie at dev_ptr with rows stride_samples apart."""
+    lib = load()
+    cfg = Config()
+    lib.aisgpu_default_config(C.byref(cfg))
+    cfg.sample_rate, cfg.model, cfg.dsk, cfg.fp_ds, cfg.format = sample_rate, model, int(dsk), int(fp_ds), fmt
+    cfg.channel_mode, cfg.n_streams = channel_mode, n_streams
+    rc = lib.aisgpu_check_device_batch(C.byref(cfg), C.c_void_p(dev_ptr), stride_samples)
+    if rc:
+        raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode()))
 
 
 def make_msg(payload_bytes, nbits, channel="A", start_idx=0, end_idx=0, level=0.0, ppm=0.0, sentences=()):

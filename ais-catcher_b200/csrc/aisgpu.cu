@@ -539,9 +539,9 @@ int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int 
 		if (e == cudaSuccess) return 0;
 		if (e != cudaErrorNotSupported) CU(e);
 	}
-	if (h->fp_ds) { // the integer CIC stages only exist in the streaming kernel
-		h->err = "FP_DS on: n_samples must be a multiple of 16384 and the batch 16-byte aligned";
-		return AISGPU_EINVAL;
+	if (h->fp_ds) { // the integer CIC stages only exist in the streaming kernel; check_placement and the granule make it take every valid block
+		h->err = "internal: the FP_DS streaming front end declined the block";
+		return AISGPU_ECUDA;
 	}
 	const size_t smem = (size_t)p.smem_f2 * sizeof(float2);
 	CU(launch_frontend_tiled(p, h->in_fmt, h->k, false, dim3(n_seg, B), smem, h->fe_stream));
@@ -782,8 +782,7 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 	// ---- front-end history for the next submit (none for the FM-discriminator input's split) ----
 	if (h->P) {
 		const int nxt = h->tail_cur ^ 1;
-		const int p_w = h->P * h->bps / 8;
-		CU(launch_tail_update(h->d_tail[nxt], h->d_tail[h->tail_cur], dev_in, stride * h->bps / 8, (long long)N * h->bps / 8, p_w, B, h->fe_stream));
+		CU(launch_tail_update(h->d_tail[nxt], h->d_tail[h->tail_cur], dev_in, stride * h->bps, (long long)N * h->bps, h->P * h->bps, B, h->fe_stream));
 		h->tail_cur = nxt;
 		h->last_launches++;
 	}
@@ -910,6 +909,10 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 	return 0;
 }
 
+// DownsampleKFilter::Receive returns at once on a block shorter than its taps minus one (DSP.cpp:165-166): the block is dropped and the
+// filter's history, phase and output block stay as they were.  The callers skip the filter and its history update then.
+bool dsk_takes(int N) { return N >= DSK_T - 1; }
+
 // DownsampleKFilter over N input samples per stream (any format) -> ring of 96 kS/s samples
 int run_dsk(aisgpu_handle *h, const void *in, long long stride, int fmt, int N, const void *tail, float2 *S, long long s_stride, long long &produced, int cap) {
 	const int B = h->cfg.n_streams;
@@ -940,6 +943,43 @@ int check_outer(aisgpu_handle *h, int N) {
 	}
 	if ((h->pre == 1 || h->pre == 3) && h->outer_N && N != h->outer_N) {
 		h->err = "at an interpolated sample rate every submit must have the same length (DSP::Upsample re-blocks by it, DSP.cpp:203)";
+		return AISGPU_EINVAL;
+	}
+	return 0;
+}
+
+// Where a device batch (aisgpu_submit_device) may lie, from what the readers of the planned chain load:
+//  - the tiled front end and pre-stage (fe_tiled.cu) load pairs of samples at even indices with one vector load of two samples
+//    (fe_common.cuh) and copy CF32 tiles with cp.async.bulk, which needs 16-byte sources: base aligned to two samples, even stride;
+//  - the streaming kernels (fe_stream.cuh) are only chosen for 16-byte rows; the integer front end of FP_DS and single-channel
+//    mode (fe_x.cu) exist only as such kernels: base and rows 16-byte aligned, and FP_DS's lane offsets fit 32 bits of 16-byte units;
+//  - the FM-discriminator split at 48 kHz (fe_disc.cu) loads single samples where pairs are not aligned: any sample-aligned base;
+//  - DownsampleKFilter (k_dsk) and the warm-up tail copy (k_tail_update) read single samples.
+int check_placement(aisgpu_handle *h, const void *dev, int64_t stride) {
+	const unsigned long long a = (unsigned long long)(size_t)dev;
+	const int bps = bytes_per_sample(h->cfg.format);
+	if (stride < 0 || (stride & 1)) {
+		h->err = "stride_samples must be even and non-negative";
+		return AISGPU_EINVAL;
+	}
+	if (h->xmode || h->fp_ds) {
+		if (a % 16 || (stride * bps) % 16) {
+			h->err = h->xmode ? "single-channel mode: the rows of a device batch must be 16-byte aligned"
+							  : "FP_DS on: the rows of a device batch must be 16-byte aligned";
+			return AISGPU_EINVAL;
+		}
+		if (h->fp_ds && (unsigned long long)h->cfg.n_streams * (unsigned long long)stride * (unsigned long long)bps >= (1ull << 36)) {
+			h->err = "FP_DS on: a device batch must span less than 64 GiB";
+			return AISGPU_EINVAL;
+		}
+		return 0;
+	}
+	const int align = (h->disc && h->pre == 0) ? bps : 2 * bps;
+	if (a % align) {
+		char b[160];
+		snprintf(b, sizeof(b), "the base of a device batch must be aligned to %d bytes (%s)", align,
+				 align == bps ? "one sample" : "two samples");
+		h->err = b;
 		return AISGPU_EINVAL;
 	}
 	return 0;
@@ -1009,10 +1049,12 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 			tail_len = h->PA;
 			if (h->pre == 4) { // the level-kA stream goes straight through DownsampleKFilter into the 96 kS/s ring
 				const int c2 = h->ptail2_cur;
-				if ((rc = run_dsk(h, h->d_D0 + 2, h->d0_stride, AISGPU_FMT_CF32, L, h->d_ptail2[c2], h->d_S, h->s_stride, h->s_produced, h->s_cap))) return rc;
-				CU(launch_tail_update(h->d_ptail2[c2 ^ 1], h->d_ptail2[c2], h->d_D0 + 2, h->d0_stride, (long long)L, 32, B, h->fe_stream));
-				h->ptail2_cur = c2 ^ 1;
-				h->last_launches += 2;
+				if (dsk_takes(L)) {
+					if ((rc = run_dsk(h, h->d_D0 + 2, h->d0_stride, AISGPU_FMT_CF32, L, h->d_ptail2[c2], h->d_S, h->s_stride, h->s_produced, h->s_cap))) return rc;
+					CU(launch_tail_update(h->d_ptail2[c2 ^ 1], h->d_ptail2[c2], h->d_D0 + 2, h->d0_stride * 8, (long long)L * 8, 32 * 8, B, h->fe_stream));
+					h->ptail2_cur = c2 ^ 1;
+					h->last_launches += 2;
+				}
 			}
 			else {
 			// replay Upsample's float accumulator: one (input index, alpha) pair per output (DSP.cpp:196-209).  The table goes
@@ -1054,8 +1096,7 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 			if ((rc = run_dsk(h, dev_in, stride, h->cfg.format, N, h->d_ptail[cur], h->d_S, h->s_stride, h->s_produced, h->s_cap))) return rc;
 		}
 		{ // raw-format history of the pre-stage for the next submit
-			const int p_w = tail_len * h->obps / 8;
-			CU(launch_tail_update(h->d_ptail[nxt], h->d_ptail[cur], dev_in, stride * h->obps / 8, (long long)N * h->obps / 8, p_w, B, h->fe_stream));
+			CU(launch_tail_update(h->d_ptail[nxt], h->d_ptail[cur], dev_in, stride * h->obps, (long long)N * h->obps, tail_len * h->obps, B, h->fe_stream));
 			h->ptail_cur = nxt;
 			h->last_launches++;
 		}
@@ -1063,9 +1104,11 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 			while (h->s_produced - h->s_consumed >= h->us_blk) {
 				const int slot = (int)(h->s_consumed % h->s_cap);
 				const int c2 = h->ptail2_cur;
-				if ((rc = run_dsk(h, h->d_S + slot, h->s_stride, AISGPU_FMT_CF32, h->us_blk, h->d_ptail2[c2], h->d_S2, h->s2_stride, h->s2_produced, h->s2_cap))) return rc;
-				CU(launch_tail_update(h->d_ptail2[c2 ^ 1], h->d_ptail2[c2], h->d_S + slot, h->s_stride, (long long)h->us_blk, 32, B, h->fe_stream));
-				h->ptail2_cur = c2 ^ 1;
+				if (dsk_takes(h->us_blk)) {
+					if ((rc = run_dsk(h, h->d_S + slot, h->s_stride, AISGPU_FMT_CF32, h->us_blk, h->d_ptail2[c2], h->d_S2, h->s2_stride, h->s2_produced, h->s2_cap))) return rc;
+					CU(launch_tail_update(h->d_ptail2[c2 ^ 1], h->d_ptail2[c2], h->d_S + slot, h->s_stride * 8, (long long)h->us_blk * 8, 32 * 8, B, h->fe_stream));
+					h->ptail2_cur = c2 ^ 1;
+				}
 				h->s_consumed += h->us_blk;
 			}
 			while (h->s2_produced - h->s2_consumed >= h->blk) {
@@ -1646,12 +1689,9 @@ static int poison(aisgpu_handle *h, int rc) {
 int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stride_samples, int n_samples) {
 	ENTER(h);
 	if (!dev_samples) return AISGPU_EINVAL;
-	if (stride_samples < n_samples || (stride_samples & 1)) {
-		h->err = "stride_samples must be even and >= n_samples";
-		return AISGPU_EINVAL;
-	}
-	if (h->xmode && (((size_t)dev_samples % 16) != 0 || ((stride_samples * h->obps) % 16) != 0)) {
-		h->err = "single-channel mode: the rows of a device batch must be 16-byte aligned";
+	if (int rc = check_placement(h, dev_samples, stride_samples)) return rc;
+	if (stride_samples < n_samples) {
+		h->err = "stride_samples must be >= n_samples";
 		return AISGPU_EINVAL;
 	}
 	if (int rc = check_outer(h, n_samples)) return rc; // all argument checks come before any state is touched
@@ -1989,6 +2029,24 @@ int aisgpu_chunk_granule(const aisgpu_config *cfg) {
 		return rc;
 	}
 	return outer_granule(&tmp);
+}
+
+int aisgpu_check_device_batch(const aisgpu_config *cfg, const void *dev_samples, int64_t stride_samples) {
+	aisgpu_config c;
+	if (!copy_config(cfg, &c) || !dev_samples) {
+		g_create_error = "aisgpu_check_device_batch: null argument or struct_size mismatch";
+		return AISGPU_EINVAL;
+	}
+	if (c.format < 0 || c.format > 3 || c.n_streams < 1) {
+		g_create_error = "bad format / n_streams";
+		return AISGPU_EINVAL;
+	}
+	aisgpu_handle tmp;
+	tmp.cfg = c;
+	int rc = plan_frontend(&tmp);
+	if (!rc) rc = check_placement(&tmp, dev_samples, stride_samples);
+	if (rc) g_create_error = tmp.err;
+	return rc;
 }
 
 int aisgpu_validate(const uint8_t *data, int nbits) {

@@ -78,14 +78,17 @@ __global__ void __launch_bounds__(DSK_THREADS) k_dsk(const void *__restrict__ in
 	S[(long long)stream * s_stride + (int)((j0 + o) % cap)] = acc;
 }
 
-// new_tail = last P samples of (old_tail ++ chunk); works for any N.  Copies 8-byte words (P is a multiple of 4
-// samples and every format has >= 2 bytes per sample, so rows and offsets stay 8-byte aligned).
-__global__ void k_tail_update(uint2 *__restrict__ new_tail, const uint2 *__restrict__ old_tail, const uint2 *__restrict__ in,
-							  long long in_stride_w, long long n_w, int p_w) {
+// new_tail = last P samples of (old_tail ++ chunk); works for any N.  Copies words of sizeof(W) bytes: the launcher picks the
+// widest word that divides the input's base, its row stride, N and P in bytes.  A device batch's row stride is any even number of
+// samples (aisgpu_check_device_batch), which for CU8 / CS8 is a multiple of 4 bytes but not always of 8.
+template <typename W>
+__global__ void k_tail_update(W *__restrict__ new_tail, const W *__restrict__ old_tail, const unsigned char *__restrict__ in,
+							  long long in_stride_b, long long n_w, int p_w) {
 	const int stream = blockIdx.y;
+	const W *row = reinterpret_cast<const W *>(in + (long long)stream * in_stride_b);
 	for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < p_w; i += gridDim.x * blockDim.x) {
 		const long long s = (long long)i + n_w - p_w; // word index relative to chunk start
-		new_tail[(long long)stream * p_w + i] = s >= 0 ? in[(long long)stream * in_stride_w + s] : old_tail[(long long)stream * p_w + (s + p_w)];
+		new_tail[(long long)stream * p_w + i] = s >= 0 ? row[s] : old_tail[(long long)stream * p_w + (s + p_w)];
 	}
 }
 
@@ -142,10 +145,19 @@ cudaError_t launch_dsk(int fmt, const void *in, long long in_stride, const void 
 	}
 	return cudaGetLastError();
 }
-cudaError_t launch_tail_update(void *new_tail, const void *old_tail, const void *in, long long in_stride_w, long long n_w, int p_w, int B, cudaStream_t s) {
+template <typename W>
+static cudaError_t tail_update_w(void *new_tail, const void *old_tail, const void *in, long long in_stride_b, long long n_b, int p_b, int B, cudaStream_t s) {
+	const int p_w = p_b / (int)sizeof(W);
 	dim3 grid((p_w + 127) / 128, B);
-	k_tail_update<<<grid, 128, 0, s>>>((uint2 *)new_tail, (const uint2 *)old_tail, (const uint2 *)in, in_stride_w, n_w, p_w);
+	k_tail_update<W><<<grid, 128, 0, s>>>((W *)new_tail, (const W *)old_tail, (const unsigned char *)in, in_stride_b, n_b / (long long)sizeof(W), p_w);
 	return cudaGetLastError();
+}
+cudaError_t launch_tail_update(void *new_tail, const void *old_tail, const void *in, long long in_stride_b, long long n_b, int p_b, int B, cudaStream_t s) {
+	const unsigned long long m = (unsigned long long)(size_t)in | (unsigned long long)in_stride_b | (unsigned long long)n_b | (unsigned long long)p_b;
+	if (m % 8 == 0) return tail_update_w<uint2>(new_tail, old_tail, in, in_stride_b, n_b, p_b, B, s);
+	if (m % 4 == 0) return tail_update_w<unsigned>(new_tail, old_tail, in, in_stride_b, n_b, p_b, B, s);
+	if (m % 2 == 0) return tail_update_w<unsigned short>(new_tail, old_tail, in, in_stride_b, n_b, p_b, B, s);
+	return tail_update_w<unsigned char>(new_tail, old_tail, in, in_stride_b, n_b, p_b, B, s);
 }
 cudaError_t launch_carry_f2(float2 *buf, long long stride, int src_begin, int dst_begin, int cnt, int rows, cudaStream_t s) {
 	k_carry<float2><<<rows, 128, cnt * sizeof(float2), s>>>(buf, stride, src_begin, dst_begin, cnt);

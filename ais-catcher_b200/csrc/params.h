@@ -176,7 +176,8 @@ cudaError_t launch_upsample(const float2 *D0, long long d0_stride, int d0_off, c
 cudaError_t launch_d0_carry(float2 *D0, long long d0_stride, int d0_off, int L, int rows, cudaStream_t s);
 cudaError_t launch_dsk(int fmt, const void *in, long long in_stride, const void *tail, int tail_len, int first, int n_out, int B, float2 *S, long long s_stride,
                        long long j0, int cap, cudaStream_t s);
-cudaError_t launch_tail_update(void *new_tail, const void *old_tail, const void *in, long long in_stride_w, long long n_w, int p_w, int B, cudaStream_t s);
+// last p_b bytes of (old_tail ++ the first n_b bytes of each input row) -> new_tail; rows of `in` are in_stride_b bytes apart
+cudaError_t launch_tail_update(void *new_tail, const void *old_tail, const void *in, long long in_stride_b, long long n_b, int p_b, int B, cudaStream_t s);
 cudaError_t launch_carry_f2(float2 *buf, long long stride, int src_begin, int dst_begin, int cnt, int rows, cudaStream_t s);
 cudaError_t launch_carry2_f2(const float2 *src, float2 *dst, long long stride, int src_begin, int dst_begin, int cnt, int rows, cudaStream_t s);
 cudaError_t set_taps_bh28_3(const float *taps26);

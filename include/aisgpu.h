@@ -167,8 +167,19 @@ int aisgpu_submit_v(aisgpu_handle *h, const void *const *stream_ptrs, int n_samp
  * step c - 1. */
 int aisgpu_submit_async(aisgpu_handle *h, const void *host_samples, int n_samples, int64_t *ticket);
 
-/* Same, with the batch already resident in device memory ([n_streams][stride_samples], first n_samples used). */
+/* Same, with the batch already resident in device memory ([n_streams][stride_samples], first n_samples used).  n_samples may
+ * change from call to call as for aisgpu_submit, and so may dev_samples and stride_samples.  Placement rule (checked by
+ * aisgpu_check_device_batch, which this calls first; a batch that breaks it is AISGPU_EINVAL with the handle untouched):
+ *   - stride_samples is even and >= n_samples;
+ *   - dev_samples is aligned to two samples: 16 bytes for CF32, 8 for CS16, 4 for CU8 / CS8;
+ *   - AISGPU_MODE_X and FP_DS: dev_samples and every row are 16-byte aligned (stride_samples * bytes per sample % 16 == 0);
+ *   - AISGPU_MODEL_DISCRIMINATOR at exactly 48000 S/s: dev_samples only needs to be aligned to one sample. */
 int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stride_samples, int n_samples);
+
+/* The placement rule of aisgpu_submit_device for an engine created with *cfg, without touching the GPU (dev_samples is only
+ * inspected as a number): 0 if the batch may lie there, else AISGPU_EINVAL (also for a configuration aisgpu_create refuses) with
+ * the reason in aisgpu_last_error(NULL).  stride_samples >= n_samples is aisgpu_submit_device's own check. */
+int aisgpu_check_device_batch(const aisgpu_config *cfg, const void *dev_samples, int64_t stride_samples);
 
 /* Waits for all submitted work (cudaStreamSynchronize). */
 int aisgpu_sync(aisgpu_handle *h);

@@ -95,6 +95,88 @@ def test_product_never_touches_the_oracle():
         assert b"aisorc_" not in blob and b"aisref_" not in blob
 
 
+# ---- placement rule of a device batch (aisgpu_check_device_batch, host-only) -------------------------------------------
+
+BASE = 0x7F0000000000  # a device-looking address, 4 KiB aligned; the rule only looks at the number
+AB, X = aisgpu.MODE_AB, aisgpu.MODE_X
+CF32, CU8, CS8, CS16 = aisgpu.FMT_CF32, aisgpu.FMT_CU8, aisgpu.FMT_CS8, aisgpu.FMT_CS16
+M0, M2, M3, M4, M11 = aisgpu.MODEL_STANDARD, aisgpu.MODEL_DEFAULT, aisgpu.MODEL_DISCRIMINATOR, aisgpu.MODEL_CHALLENGER, aisgpu.MODEL_V2
+
+# (model, rate, format, channel mode, dsk, fp_ds) -> [(base offset in bytes, stride in samples, accepted)]
+N = 65536
+PLACEMENT = [
+    # AB, exact buckets: the base aligned to two samples, any even stride (streaming kernel for 16-byte rows, tiled otherwise)
+    ((M2, 1536000, CF32, AB, 0, 0), [(0, N, 1), (16, N + 2, 1), (8, N, 0), (4, N, 0), (0, N + 1, 0), (0, -2, 0), (32, 3 * N, 1)]),
+    ((M0, 1536000, CU8, AB, 0, 0), [(0, N, 1), (4, N + 2, 1), (4, N + 6, 1), (2, N, 0), (1, N, 0), (0, N + 1, 0)]),
+    ((M4, 1536000, CS8, AB, 0, 0), [(4, N + 2, 1), (8, N + 64, 1), (2, N + 2, 0), (3, N, 0)]),
+    ((M11, 1536000, CS16, AB, 0, 0), [(8, N + 2, 1), (16, N + 4, 1), (4, N, 0), (2, N, 0)]),
+    ((M2, 384000, CF32, AB, 0, 0), [(16, N + 2, 1), (8, N + 2, 0)]),
+    ((M2, 12288000, CU8, AB, 0, 0), [(4, N + 2, 1), (2, N + 2, 0)]),
+    # pre-stages: Upsample (6 MS/s: 4 CIC stages in front of it), DownsampleKFilter (288k on the raw input, 1152k behind CIC stages)
+    ((M2, 6000000, CF32, AB, 0, 0), [(16, N + 2, 1), (8, N, 0)]),
+    ((M0, 6000000, CU8, AB, 0, 0), [(4, N + 6, 1), (2, N, 0)]),
+    ((M2, 288000, CS16, AB, 0, 0), [(8, N + 2, 1), (4, N, 0)]),
+    ((M2, 288000, CU8, AB, 1, 0), [(4, N + 2, 1), (2, N, 0)]),
+    ((M0, 1152000, CF32, AB, 1, 0), [(16, N + 2, 1), (8, N + 2, 0)]),
+    # FP_DS: the integer front end only exists as the streaming kernel: 16-byte base and rows (CU8: strides of 8 samples)
+    ((M2, 1536000, CU8, AB, 0, 1), [(0, N, 1), (16, N + 8, 1), (4, N, 0), (8, N, 0), (0, N + 2, 0), (0, N + 6, 0), (0, N + 4, 0)]),
+    # single-channel mode: 16-byte base and rows at every rate, the interpolated ones included
+    ((M2, 96000, CF32, X, 0, 0), [(0, N, 1), (16, N + 2, 1), (8, N, 0)]),
+    ((M0, 192000, CU8, X, 0, 0), [(16, N + 8, 1), (0, N + 2, 0), (4, N, 0)]),
+    ((M4, 48000, CS16, X, 0, 0), [(16, N + 4, 1), (0, N + 2, 0), (8, N, 0)]),
+    ((M2, 44100, CF32, X, 0, 0), [(16, N + 2, 1), (8, N + 2, 0)]),
+    # FM-discriminator input: any sample-aligned base at 48 kHz (the split loads single samples there), two samples behind Upsample
+    ((M3, 48000, CF32, AB, 0, 0), [(8, N + 2, 1), (16, N, 1), (4, N, 0), (8, N + 1, 0)]),
+    ((M3, 48000, CU8, AB, 0, 0), [(2, N + 2, 1), (1, N, 0)]),
+    ((M3, 48000, CS16, X, 0, 0), [(4, N + 6, 1), (2, N, 0)]),
+    ((M3, 44100, CU8, AB, 0, 0), [(4, N + 2, 1), (2, N, 0)]),
+    ((M3, 12000, CF32, AB, 0, 0), [(16, N + 2, 1), (8, N, 0)]),
+]
+
+
+def placement_ok(cfg, off, stride):
+    model, fs, fmt, mode, dsk, fp_ds = cfg
+    try:
+        aisgpu.check_device_batch(BASE + off, stride, sample_rate=fs, model=model, fmt=fmt, dsk=dsk, fp_ds=fp_ds, channel_mode=mode)
+    except aisgpu.AisGpuError as e:
+        assert "rc=-1" in str(e) and len(str(e)) > 12, e  # EINVAL with the reason
+        return 0
+    return 1
+
+
+@pytest.mark.parametrize("cfg,cases", PLACEMENT, ids=["m%d_%d_f%d_mode%d_dsk%d_fpds%d" % c for c, _ in PLACEMENT])
+def test_device_batch_placement_rule(built, cfg, cases):
+    got = [(off, stride, placement_ok(cfg, off, stride)) for off, stride, _ in cases]
+    assert got == cases
+
+
+def test_device_batch_placement_rule_refusals(built):
+    lib = aisgpu.load()
+    # the engine's own configuration errors, with the same wording as aisgpu_create
+    with pytest.raises(aisgpu.AisGpuError, match="between 96K and 12288K"):
+        aisgpu.check_device_batch(BASE, N, sample_rate=48000)
+    with pytest.raises(aisgpu.AisGpuError, match="needs CU8"):
+        aisgpu.check_device_batch(BASE, N, fmt=CF32, fp_ds=True)
+    with pytest.raises(aisgpu.AisGpuError, match="16-byte"):
+        aisgpu.check_device_batch(BASE + 8, N, fmt=CU8, fp_ds=True)
+    with pytest.raises(aisgpu.AisGpuError, match="two samples"):
+        aisgpu.check_device_batch(BASE + 2, N, fmt=CU8)
+    # FP_DS lane offsets are 32-bit counts of 16-byte units: the whole batch must span less than 64 GiB
+    aisgpu.check_device_batch(BASE, 1 << 24, fmt=CU8, fp_ds=True, n_streams=1024)
+    with pytest.raises(aisgpu.AisGpuError, match="64 GiB"):
+        aisgpu.check_device_batch(BASE, 1 << 25, fmt=CU8, fp_ds=True, n_streams=1024)
+    cfg = aisgpu.Config()
+    lib.aisgpu_default_config(C.byref(cfg))
+    assert lib.aisgpu_check_device_batch(C.byref(cfg), None, N) == aisgpu.EINVAL
+    assert lib.aisgpu_check_device_batch(None, C.c_void_p(BASE), N) == aisgpu.EINVAL
+    cfg.format = 9
+    assert lib.aisgpu_check_device_batch(C.byref(cfg), C.c_void_p(BASE), N) == aisgpu.EINVAL
+    # a caller built before channel_mode existed gets AB
+    lib.aisgpu_default_config(C.byref(cfg))
+    cfg.struct_size = aisgpu.Config.channel_mode.offset
+    assert lib.aisgpu_check_device_batch(C.byref(cfg), C.c_void_p(BASE + 16), N + 2) == 0
+
+
 # ---- host-only per-frame tail -------------------------------------------------------------------------------------
 
 def pack(bits):

@@ -25,10 +25,12 @@ def case(name, model, fs, N, nchunks, **kw):
     return name
 
 
-def digest(Model, model, fs, N, nchunks, fmt=O.FMT_CF32, flags=O.DEFAULT_FLAGS, seed=0, multi=False):
+def digest(Model, model, fs, N, nchunks, fmt=O.FMT_CF32, flags=O.DEFAULT_FLAGS, seed=0, multi=False, schedule=None):
     """Runs one model over the seeded stimulus; returns the input hash, one hash over every tap of every chunk (in order,
-    with lengths) and the per-chunk message records."""
-    x = S.random_stream(fs, N * nchunks, seed, multi_sentence=multi)[0]
+    with lengths) and the per-chunk message records.  schedule: the length of every chunk (instead of nchunks chunks of N)."""
+    lengths = list(schedule) if schedule is not None else [N] * nchunks
+    offs = np.cumsum([0] + lengths)
+    x = S.random_stream(fs, int(offs[-1]), seed, multi_sentence=multi)[0]
     per = 1
     if fmt == O.FMT_CU8:
         x, per = S.to_cu8(x), 2
@@ -41,8 +43,8 @@ def digest(Model, model, fs, N, nchunks, fmt=O.FMT_CF32, flags=O.DEFAULT_FLAGS, 
     m = Model(model=model, sample_rate=fs, fmt=fmt, flags=flags, taps=True)
     h = hashlib.sha256()
     msgs = []
-    for c in range(nchunks):
-        blk = x[c * N * per:(c + 1) * N * per]
+    for c in range(len(lengths)):
+        blk = x[offs[c] * per:offs[c + 1] * per]
         m.push(blk)
         taps = [m.tap_c(t) for t in range(9)] + [m.tap_f(t) for t in range(14)] + [m.tap_ppm(t) for t in (O.TAP_CGF_A, O.TAP_CGF_B)]
         for a in taps:
@@ -81,6 +83,13 @@ FLAGS = {f: case("flag_variants_%d" % f, O.MODEL_DEFAULT, 1536000, 32768, 6, fla
          for f in (O.FLAG_AFC_WIDE | O.FLAG_DROOP, O.FLAG_PS_EMA, O.FLAG_PS_EMA | O.FLAG_DROOP, 0)}
 SMALL = [case("small_chunks_m%d" % m, m, 1536000, 4096, 48, seed=7) for m in (O.MODEL_DEFAULT, O.MODEL_STANDARD)]
 MULTI = case("multi_sentence", O.MODEL_DEFAULT, 1536000, 65536, 6, seed=31, multi=True)
+# one stream, the chunk length changing from push to push (in granules of the rate: 64 at 1536k): a chunk shorter than the
+# front end's history, chunks either side of a 48 kHz CGF block (256 granules), one granule, a long one, no power of two
+SCHEDULE = [5, 24, 23, 1024, 1, 257, 255, 1017, 613, 1]
+SCHED_RATES = {1536000: 64, 96000: 4, 6144000: 256}
+SCHEDULES = {(m, fs, f): case("schedule_m%d_%d_f%d" % (m, fs, f), m, fs, 0, 0, fmt=f, seed=61, schedule=[g * u for u in SCHEDULE])
+             for m in (O.MODEL_DEFAULT, O.MODEL_STANDARD, O.MODEL_BASE) for fs, g in SCHED_RATES.items()
+             for f in ((O.FMT_CF32, O.FMT_CU8) if fs == 1536000 else (O.FMT_CF32,))}
 
 
 @pytest.mark.parametrize("model", [O.MODEL_DEFAULT, O.MODEL_STANDARD, O.MODEL_BASE])
@@ -116,6 +125,12 @@ def test_multi_sentence(built):
     # 424-bit messages -> two sentences with the sequence id of Message.cpp:28-39
     n = compare(MULTI)
     assert n >= 2
+
+
+@pytest.mark.parametrize("key", sorted(SCHEDULES), ids=lambda k: "m%d_%d_f%d" % k)
+def test_changing_chunk_lengths(built, key):
+    # the GPU tests of changing submit lengths fall back on the port where the reference was not built
+    assert compare(SCHEDULES[key]) >= 1
 
 
 if __name__ == "__main__":  # regenerate the stored outputs from the reference (needs oracle/_ref)

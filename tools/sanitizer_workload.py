@@ -56,6 +56,29 @@ for fs_d, fmt in ((48000, aisgpu.FMT_CS16), (44100, aisgpu.FMT_CF32)):  # FM-dis
         eng.submit(np.stack([x[c * nd * per:(c + 1) * nd * per] for x in xd]), nd)
     print("-m 3", fs_d, "messages", len(eng.poll()))
     eng.close()
+sched = [320, 1536, 1472, 16384 + 64, 64, 16384 - 64, 64 * 1017]  # one engine, the submit length changing (tiled <-> streaming)
+xv = np.stack([aissynth.random_stream(fs, sum(sched), 700 + s)[0] for s in range(B)])
+eng = aisgpu.Engine(model=aisgpu.MODEL_DEFAULT, sample_rate=fs, n_streams=B, max_chunk=max(sched))
+o = 0
+for n in sched:
+    eng.submit(np.ascontiguousarray(xv[:, o:o + n]), n)
+    o += n
+print("length schedule messages", len(eng.poll()))
+eng.close()
+import torch  # CU8 device batch with padded rows (N + 2, N + 6: not a multiple of 8 bytes) and a base 2 samples in
+cu = np.stack([aissynth.to_cu8(x) for x in xs])
+eng = aisgpu.Engine(model=aisgpu.MODEL_STANDARD, sample_rate=fs, fmt=aisgpu.FMT_CU8, n_streams=B, max_chunk=N, host_staging=False)
+for c, (stride, off) in enumerate(((N + 2, 0), (N + 6, 4), (N + 2, 4), (N + 6, 0))):
+    host = np.zeros(off + B * stride * 2, np.uint8)
+    for s in range(B):
+        host[off + s * stride * 2:off + s * stride * 2 + N * 2] = cu[s, c * N * 2:(c + 1) * N * 2]
+    dev = torch.from_numpy(host).cuda()
+    torch.cuda.synchronize()
+    eng.submit_device(dev.data_ptr() + off, stride, N)
+    eng.sync()
+    del dev
+print("padded-stride CU8 device batch messages", len(eng.poll()))
+eng.close()
 with tempfile.TemporaryDirectory() as d:  # file feeder, CU8, ragged lengths, FP_DS integer front end
     paths = []
     for s in range(2):
