@@ -62,6 +62,12 @@ constexpr int V2_BLK = 512; // V2::BLOCK_SIZE (V2Engine.h:30)
 constexpr int HD = 48;  // ModelChallenger: derotated samples kept in front of the new ones (FM needs 1, FIR37 36, a partial group 4)
 constexpr int HE = 8;   // room in front of new symbol-stage samples: an incomplete group of 5 (<=4)
 
+// the tiled front end (the CIC stages below 768 kS/s, and of blocks the streaming kernel declines): input samples per tile --
+// one run of 5 outputs per thread of a four-warp CTA at the first CIC stage, 2 x 5 x 128 -- and the CTAs a submit is cut into
+// (segments x streams, several waves over the SMs)
+constexpr int FE_TILE = 1280;
+constexpr int FE_CTAS = 4096;
+
 constexpr int X_GRANULE = 64; // single-channel mode: a multiple of every format's front-end lane chunk (frontend_x_granule); also the
                               // FM-discriminator input model's granule
 
@@ -71,7 +77,7 @@ int bytes_per_sample(int fmt) { return fmt == AISGPU_FMT_CF32 ? 8 : (fmt == AISG
 
 struct aisgpu_handle {
 	aisgpu_config cfg;
-	int k = 0, P = 0, P96 = 0, tile = 0, bps = 8;
+	int k = 0, P = 0, P96 = 0, bps = 8;
 	// Rates the reference serves through DSP::Upsample (non-bucket rates, Model.cpp:134-149) or DSP::DownsampleKFilter
 	// (288 kS/s, Model.cpp:308-313) get a pre-stage that fills a ring of whole reference blocks (d_S); the front end
 	// proper then runs once per block with k = the CIC stages behind the resampler ("inner" submits).
@@ -94,7 +100,6 @@ struct aisgpu_handle {
 	int *d_us_src = nullptr;
 	float *d_us_alpha = nullptr;
 	FeParams fe_pre;
-	int pre_tile = 0;
 	long long msg_chunk = 0; // ordinal of the caller's submit (what frames are tagged with)
 	long long pre_tap0 = 0, pre_tap1 = 0, pre2_tap0 = 0, pre2_tap1 = 0; // resampler outputs of the last submit (ring positions), for AISGPU_TAP_PRE / _PRE2
 	int obps = 8;            // bytes per sample of the caller's format (bps: of what the front end proper reads)
@@ -107,10 +112,8 @@ struct aisgpu_handle {
 	float fdc_alpha = 0, fdc_beta = 1;
 	int rows = 0;
 	int max_n48 = 0;
-	int fe_warps = 4, fe_tile = 0, fe_ctas = 4096;
-	int fe_st = 1, st_L = 0, st_ring = 0, st_kmax = 7; // AISGPU_FE_ST=0 disables the per-thread streaming kernel; AISGPU_ST_L: lanes per stream (0: the launcher plans); AISGPU_ST_NB: ring depth 3 | 5 (0: per chain)
-	int cf_rows = 8; // AISGPU_CF_ROWS: rows per CTA of the fused CGF kernel (4 or 8); 8 halves the chain warp's instructions (chosen on the previous target; not re-measured on the H100)
-	int dec_rpw = 6, decoder = 3; // rows per warp / which decoder kernel // front-end launch shape (tunable through AISGPU_FE_WARPS / _TILE / _CTAS)
+	int st_L = 0; // AISGPU_ST_L: lanes per stream of the streaming front end (0: the launcher plans)
+	int dec_rpw = 6, decoder = 3; // AISGPU_DEC_RPW: rows per warp of the word-parallel decoder; AISGPU_DECODER=1: the bit-serial one
 	// fe_stream: front end + input history; stream: everything behind the 48 kHz buffers (the stream handed to callers
 	// for timing).  The front end of submit c+1 overlaps the back end of submit c; Cbuf is double buffered for that.
 	cudaStream_t stream = nullptr, copy_stream = nullptr, fe_stream = nullptr;
@@ -490,25 +493,43 @@ int launch_frontend_split(aisgpu_handle *h, const void *dev_in, long long stride
 	return 0;
 }
 
+// The CIC stages of the AB front end over p.N samples per stream of format fmt (bps bytes per sample): k x Downsample2CIC5, then
+// [FilterComplex3Tap ->] Rotate -> per channel Downsample2CIC5 + FilterCIC5 into Cbuf; pre: only the level-k samples, into D0 in
+// front of the resampler.  The per-thread streaming kernel (768 kS/s and above) takes the block when the rows are 16-byte aligned:
+// its launcher splits every stream over as many lanes as make one balanced wave (st_plan, fe_stream.cuh) and declines a k it has
+// no shape for and blocks shorter than four warm-ups.  The tiled kernel takes the rest.
+int launch_cic(aisgpu_handle *h, FeParams &p, int fmt, int bps, int k, bool pre) {
+	const int B = h->cfg.n_streams;
+	if (((p.in_stride * bps) % 16) == 0 && (((size_t)p.in) % 16) == 0) {
+		p.st_B = B;
+		// CF32's four-warp CTAs (fe_stream_f0.cu) are planned as ONE balanced wave of one CTA per SM, chosen over power-of-two lane
+		// splits on live step times at 1024 x 131072 on the previous target (not re-measured on the H100): the rest of the SM is left
+		// to the back-end CTAs that run beside the front end of the next submit.  The integer formats' one-warp CTAs: as many as fit.
+		p.st_cap = fmt == 0 ? 1 : 0;
+		const cudaError_t e = h->fp_ds ? launch_frontend_stream_fpds(p, h->st_L, h->fe_stream) : launch_frontend_stream(p, fmt, k, pre, h->st_L, h->fe_stream);
+		if (e == cudaSuccess) return 0;
+		if (e != cudaErrorNotSupported) CU(e);
+	}
+	if (h->fp_ds) { // the integer CIC stages only exist in the streaming kernel; check_placement and the granule make it take every valid block
+		h->err = "internal: the FP_DS streaming front end declined the block";
+		return AISGPU_ECUDA;
+	}
+	const int q = 1 << (k + 2); // a tile is a whole number of super-steps
+	int tile = (FE_TILE + q - 1) / q * q;
+	if (tile > p.N) tile = p.N;
+	if (tile != p.tile) layout_frontend(p, k, tile);
+	const int tiles_total = (p.N + tile - 1) / tile;
+	const int n_seg = std::max(1, std::min((FE_CTAS + B - 1) / B, tiles_total));
+	p.seg_len = (tiles_total + n_seg - 1) / n_seg * tile;
+	const dim3 grid((p.N + p.seg_len - 1) / p.seg_len, B);
+	CU(launch_frontend_tiled(p, fmt, k, pre, grid, (size_t)p.smem_f2 * sizeof(float2), h->fe_stream));
+	return 0;
+}
+
 int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	if (h->xmode) return launch_frontend_single(h, dev_in, stride, N);
 	if (h->disc) return launch_frontend_split(h, dev_in, stride, N);
 	FeParams &p = h->fe;
-	const int q = 1 << (h->k + 2);
-	// per-CTA tile: one run of 5 outputs per thread at the first CIC stage (2 x 5 x threads input samples)
-	int tile = h->fe_tile > 0 ? h->fe_tile : 320 * h->fe_warps;
-	if (tile % q) tile = (tile / q + 1) * q;
-	if (tile > N) tile = N;
-	if (tile != p.tile) layout_frontend(p, h->k, tile);
-	h->tile = tile;
-	const int B = h->cfg.n_streams;
-	int n_seg = (h->fe_ctas + B - 1) / B; // enough CTAs for several waves over the SMs
-	int tiles_total = (N + tile - 1) / tile;
-	if (n_seg > tiles_total) n_seg = tiles_total;
-	if (n_seg < 1) n_seg = 1;
-	int tiles_per_seg = (tiles_total + n_seg - 1) / n_seg;
-	p.seg_len = tiles_per_seg * tile;
-	n_seg = (N + p.seg_len - 1) / p.seg_len;
 	p.in = dev_in;
 	p.tail = h->d_tail[h->tail_cur];
 	p.in_stride = stride;
@@ -523,29 +544,8 @@ int launch_frontend(aisgpu_handle *h, const void *dev_in, long long stride, int 
 	p.C = h->d_C2[h->chunk % aisgpu_handle::NC];
 	p.c_stride = h->c_stride;
 	p.c_off = HC;
-	// 768 kS/s and above: per-thread streaming pipeline (state in registers) when the rows are 16-byte aligned; the launcher splits
-	// every stream over as many lanes as make one balanced wave (st_plan, fe_stream.cuh) and declines blocks shorter than four warm-ups
-	if (h->fe_st && h->k >= 3 && h->k <= h->st_kmax && ((stride * h->bps) % 16) == 0 && (((size_t)dev_in) % 16) == 0) {
-		p.in = dev_in;
-		p.st_B = B;
-		p.st_first = h->chunk == 0 ? 1 : 0;
-		// CF32 launch shape: ring of 3 chunks (104 KB per CTA) + ONE balanced wave (the planner, one CTA per SM), chosen over rings
-		// of 5 and power-of-two lane splits on live step times at 1024 x 131072 on the previous target (not re-measured on the H100).
-		// The smaller ring leaves 123 KB of the SM to the back-end CTAs that run beside the front end of the next submit.
-		const int L = h->st_L;
-		p.st_ring = h->st_ring ? h->st_ring : 3;
-		p.st_cap = (h->in_fmt == 0 && !h->fp_ds) ? 1 : 0; // the integer formats run one-warp CTAs, as many per SM as fit
-		const cudaError_t e = h->fp_ds ? launch_frontend_stream_fpds(p, L, h->fe_stream) : launch_frontend_stream(p, h->in_fmt, h->k, false, L, h->fe_stream);
-		if (e == cudaSuccess) return 0;
-		if (e != cudaErrorNotSupported) CU(e);
-	}
-	if (h->fp_ds) { // the integer CIC stages only exist in the streaming kernel; check_placement and the granule make it take every valid block
-		h->err = "internal: the FP_DS streaming front end declined the block";
-		return AISGPU_ECUDA;
-	}
-	const size_t smem = (size_t)p.smem_f2 * sizeof(float2);
-	CU(launch_frontend_tiled(p, h->in_fmt, h->k, false, dim3(n_seg, B), smem, h->fe_stream));
-	return 0;
+	p.st_first = h->chunk == 0 ? 1 : 0;
+	return launch_cic(h, p, h->in_fmt, h->bps, h->k, false);
 }
 
 // stage s of this submit may start when stage s of the previous submit (other stream) has finished
@@ -843,7 +843,7 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 					if (int rc = stage_begin(h, 6)) return rc;
 				CU(launch_cgf_fused(Ccur, h->c_stride, c_begin, stepidx, h->d_steptab, h->d_cgf_rot, nblk, h->rows, h->d_fir_hist[h->fir_cur],
 									h->d_fir_hist[h->fir_cur ^ 1], h->d_Ec2[h->ec_cur], h->e_stride, HE,
-									h->d_Ed ? h->d_Ed + HD : (h->cfg.enable_taps ? h->d_tap_cgf : nullptr), h->d_Ed ? h->ed_stride : h->r_stride, h->cf_rows, h->bs));
+									h->d_Ed ? h->d_Ed + HD : (h->cfg.enable_taps ? h->d_tap_cgf : nullptr), h->d_Ed ? h->ed_stride : h->r_stride, h->bs));
 				if (int rc = stage_end(h, 1)) return rc;
 				if (int rc = stage_end(h, 2)) return rc;
 			}
@@ -1009,14 +1009,6 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 				h->s_cap = (h->us_ratio + 2) * L; // whole blocks: < L left over + up to us_ratio * L (+ a few) new samples
 			}
 			FeParams &pp = h->fe_pre;
-			int tile = 1280;
-			if (tile > N) tile = N;
-			if (tile != pp.tile) layout_frontend(pp, h->kA, tile);
-			int n_seg = (h->fe_ctas + B - 1) / B;
-			const int tiles_total = (N + tile - 1) / tile;
-			n_seg = std::max(1, std::min(n_seg, tiles_total));
-			pp.seg_len = (tiles_total + n_seg - 1) / n_seg * tile;
-			n_seg = (N + pp.seg_len - 1) / pp.seg_len;
 			pp.in = dev_in;
 			pp.tail = h->d_ptail[cur];
 			pp.in_stride = stride;
@@ -1030,22 +1022,7 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 			pp.D0 = h->d_D0;
 			pp.d0_stride = h->d0_stride;
 			pp.d0_off = 2;
-			const size_t smem = (size_t)pp.smem_f2 * sizeof(float2);
-			dim3 grid(n_seg, B);
-			bool st_done = false;
-			if (h->fe_st && h->kA >= 3 && h->kA <= 5 && ((stride * h->obps) % 16) == 0 && (((size_t)dev_in) % 16) == 0) {
-				pp.st_B = B;
-				// the decimation in front of the resampler runs the same launch shape as the front end proper (four-warp CTAs, ring of 3, one
-				// balanced wave), which was faster than one-warp CTAs with 16-sample chunks at 6 MSPS on the previous target (not re-measured
-				// on the H100)
-				pp.st_ring = h->st_ring ? h->st_ring : 3;
-				pp.st_cap = h->cfg.format == 0 ? 1 : 0;
-				const cudaError_t e = launch_frontend_stream(pp, h->cfg.format, h->kA, true, h->st_L, h->fe_stream);
-				if (e == cudaSuccess) st_done = true;
-				else if (e != cudaErrorNotSupported) CU(e);
-			}
-			if (!st_done) CU(launch_frontend_tiled(pp, h->cfg.format, h->kA, true, grid, smem, h->fe_stream));
-			if (rc) return rc;
+			if ((rc = launch_cic(h, pp, h->cfg.format, h->obps, h->kA, true))) return rc;
 			tail_len = h->PA;
 			if (h->pre == 4) { // the level-kA stream goes straight through DownsampleKFilter into the 96 kS/s ring
 				const int c2 = h->ptail2_cur;
@@ -1352,12 +1329,6 @@ static int create_impl(aisgpu_handle *h) {
 		return AISGPU_EINVAL;
 	}
 	if (int rc = plan_frontend(h)) return rc;
-	if (const char *e = getenv("AISGPU_FE_WARPS")) h->fe_warps = atoi(e);
-#ifdef AISGPU_FE_ALL_WARP_COUNTS
-	if (h->fe_warps != 2 && h->fe_warps != 8) h->fe_warps = 4;
-#else
-	h->fe_warps = 4;
-#endif
 	// rows per warp of the decoder kernel, chosen per chain on the previous target (not re-measured on the H100): the coherent
 	// chain 1; the FM chain 3 with the current front-end shape (slightly faster than 6 rows per warp)
 	h->dec_rpw = c.model == AISGPU_MODEL_DEFAULT ? 1 : (standard_tail(h) ? 3 : 6);
@@ -1365,20 +1336,11 @@ static int create_impl(aisgpu_handle *h) {
 		h->dec_rpw = atoi(e);
 		if (h->dec_rpw != 1 && h->dec_rpw != 3) h->dec_rpw = 6;
 	}
-	if (const char *e = getenv("AISGPU_DECODER")) {
-		h->decoder = atoi(e);
-		if (h->decoder != 1 && h->decoder != 2) h->decoder = 3;
-	}
-	if (const char *e = getenv("AISGPU_CF_ROWS")) h->cf_rows = atoi(e) == 8 ? 8 : 4;
+	if (const char *e = getenv("AISGPU_DECODER")) h->decoder = atoi(e) == 1 ? 1 : 3;
 	if (c.model == AISGPU_MODEL_CHALLENGER) { // ModelChallenger always demodulates with PhaseSearchEMA (Model.cpp:646-652) and needs the fused kernel's derotated output
 		h->cfg.ps_ema = 1;
 	}
-	if (const char *e = getenv("AISGPU_FE_TILE")) h->fe_tile = atoi(e);
-	if (const char *e = getenv("AISGPU_FE_ST")) h->fe_st = atoi(e) ? 1 : 0;
 	if (const char *e = getenv("AISGPU_ST_L")) h->st_L = atoi(e);
-	if (const char *e = getenv("AISGPU_ST_NB")) h->st_ring = atoi(e) == 3 ? 3 : 5;
-	if (const char *e = getenv("AISGPU_ST_KMAX")) h->st_kmax = atoi(e);
-	if (const char *e = getenv("AISGPU_FE_CTAS")) h->fe_ctas = std::max(1, atoi(e));
 	int ndev = 0;
 	if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0) {
 		h->err = "no CUDA device (the CUDA path has no CPU fallback)";
@@ -1393,10 +1355,6 @@ static int create_impl(aisgpu_handle *h) {
 	// (large-grid) front end of the next submit frees a slot, instead of queueing behind all of its CTAs.
 	int prio_lo = 0, prio_hi = 0;
 	CU(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-	int prio_mode = 1;
-	if (const char *e = getenv("AISGPU_PRIO")) prio_mode = atoi(e); // 0: one priority, 1: back end above front end, 2: the reverse (experiments)
-	if (prio_mode == 0) prio_hi = prio_lo;
-	else if (prio_mode == 2) std::swap(prio_lo, prio_hi);
 	CU(cudaStreamCreateWithPriority(&h->stream, cudaStreamNonBlocking, prio_hi));
 	h->be_streams[0] = h->be_streams[1] = h->stream;
 	{

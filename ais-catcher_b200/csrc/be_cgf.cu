@@ -102,14 +102,16 @@ __constant__ float c_taps_coherent[FIRC_T]; // FilterComplex 17 taps (Filters.h:
 // K2bc: the derotation phasor chain, output[i] *= rot and FilterComplex 17 taps in ONE kernel (DSP.cpp:457-465, 215-246).
 // The chain rot *= rot_step is strictly sequential per row (4096 dependent complex products per submit at the bench
 // shape: their latency is the floor for the whole stage), everything else is parallel.  A CTA owns CF_ROWS rows: warp 0 runs
-// the chains, one lane per row, CF_T steps ahead into a double-buffered shared tile; meanwhile the two consumer warps
+// the chains, one lane per row, CF_T steps ahead into a double-buffered shared tile; meanwhile the CF_CONS consumer warps
 // derotate the previous tile (coalesced loads of the 48 kHz samples, requested one tile ahead), and run the FIR out of a
 // shared ring that keeps the 16-sample history.  The phasors never travel through HBM (an earlier version wrote them out, 67 MB per submit, and read them back).  FIR: products
 // by scalar __fmul_rn, the (re, im) accumulation by padd (two scalar __fadd_rn): two roundings per tap, as in the reference.
 // ---------------------------------------------------------------------------------------------
 constexpr int CF_T = 64;               // samples per tile and row (a 512-block = 8 tiles)
-// CF_ROWS rows per CTA, CF_CONS = CF_ROWS / 2 consumer warps (four outputs per thread and tile): 4 rows -> 512 CTAs at 2048 rows
-// (3-4 per SM, one CTA's barrier waits overlap another's arithmetic); 8 rows halve the chain warp's share of the issue slots
+// 8 rows per CTA, CF_CONS = CF_ROWS / 2 consumer warps (four outputs per thread and tile): twice the rows of a 4-row CTA halve the
+// chain warp's share of the issue slots (chosen on the previous target; not re-measured on the H100)
+constexpr int CF_ROWS = 8;
+constexpr int CF_CONS = CF_ROWS / 2;
 constexpr int CF_DERP = 2 * CF_T + 2 * CF_T / 4; // ring row: two tiles, one pad slot after every four samples
 // ring position n (0 .. 2 CF_T - 1) -> slot: threads that own four consecutive outputs read n = 4c + i; 5c + i hits 16 different
 // 8-byte banks over a half warp
@@ -132,15 +134,13 @@ struct CfParams {
 	long long tap_stride;
 };
 
-template <int CF_ROWS>
 __global__ void __launch_bounds__(32 + 16 * CF_ROWS) k_cgf_fused(const CfParams p) {
-	constexpr int CF_CONS = CF_ROWS / 2;
 	__shared__ __align__(16) float2 rotb[2][CF_ROWS][CF_T + 2]; // +2: the chain lanes (one row each) store to different banks
 	__shared__ __align__(16) float2 der[CF_ROWS][CF_DERP]; // der[r][cf_slot((t & 1) * CF_T + j)] = derotated sample j of tile t
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const int row0 = blockIdx.x * CF_ROWS;
 	const int ntiles = p.nblk * (CGF_N / CF_T);
-	const int ct = tid - 32; // consumer thread index 0..63 (negative in the chain warp)
+	const int ct = tid - 32; // consumer thread index 0 .. 32 * CF_CONS - 1 (negative in the chain warp)
 	if (warp != 0) { // FIR history of the previous submit sits where "tile -1" would have left it
 		for (int i = ct; i < CF_ROWS * (FIRC_T - 1); i += 32 * CF_CONS) {
 			const int r = i / (FIRC_T - 1), k = i - r * (FIRC_T - 1);
@@ -257,13 +257,12 @@ cudaError_t launch_cgf_estimate(const float2 *Cbuf, long long c_stride, int c_be
 	return cudaGetLastError();
 }
 cudaError_t launch_cgf_fused(const float2 *Cbuf, long long c_stride, int c_begin, const int *stepidx, const float2 *steptab, float2 *rot_state, int nblk, int rows,
-							 const float2 *hist_old, float2 *hist_new, float2 *Ebuf, long long e_stride, int e_off, float2 *tap_cgf, long long tap_stride, int rows_per_cta, cudaStream_t s) {
+							 const float2 *hist_old, float2 *hist_new, float2 *Ebuf, long long e_stride, int e_off, float2 *tap_cgf, long long tap_stride, cudaStream_t s) {
 	CfParams p;
 	p.Cbuf = Cbuf; p.c_stride = c_stride; p.c_begin = c_begin; p.stepidx = stepidx; p.steptab = steptab; p.rot_state = rot_state;
 	p.nblk = nblk; p.rows = rows; p.hist_old = hist_old; p.hist_new = hist_new; p.Ebuf = Ebuf; p.e_stride = e_stride; p.e_off = e_off;
 	p.tap_cgf = tap_cgf; p.tap_stride = tap_stride;
-	if (rows_per_cta == 8) k_cgf_fused<8><<<(rows + 7) / 8, 32 + 16 * 8, 0, s>>>(p);
-	else k_cgf_fused<4><<<(rows + 3) / 4, 32 + 16 * 4, 0, s>>>(p);
+	k_cgf_fused<<<(rows + CF_ROWS - 1) / CF_ROWS, 32 + 16 * CF_ROWS, 0, s>>>(p);
 	return cudaGetLastError();
 }
 

@@ -114,9 +114,8 @@ __device__ __forceinline__ void st_read_pair(const unsigned char *slot, int j, c
 	}
 }
 
-// ST_WARPS: warps per CTA (independent of each other).  One-warp CTAs with a ring of 6 chunks (27.6 KB for CF32) let eight
-// CTAs share an SM and let the block scheduler spread B x st_wps warps evenly over the SMs (1024 warps on 132: 7.8 avg);
-// the 4-warp / ring-of-8 shape (147 KB per CTA, one CTA per SM) is the earlier shape, kept for A/B.
+// ST_WARPS: warps per CTA (independent of each other), ST_NB: chunks in each warp's staging ring.  CF32 runs four-warp CTAs with
+// 32-sample chunks and a ring of 3 (104 KB per CTA); the integer formats one-warp CTAs with 16-sample chunks and a ring of 8.
 // ST_G: samples a lane fetches per visit of its sub-segment.  Every lane is an independent sequential stream for DRAM (1024 warps
 // = 32768 streams, far more than there are banks), so the bytes per visit decide the row-buffer locality: 16 samples = one
 // 128-byte line per visit, 64 samples = four consecutive lines.
@@ -349,6 +348,25 @@ static inline bool st_plan(long long B, int nss, int warm, int wpc, int slots, i
 	r = nss - q * L;
 	return true;
 }
+// SMs x resident CTAs of one kernel instantiation, and the SM count: asked once per process and instantiation (the caller's
+// static cache; all devices of a box are alike)
+struct CtaSlots { std::atomic<int> slots{0}, sms{0}; };
+template <typename Kernel>
+static cudaError_t cta_slots(CtaSlots &cache, Kernel *kernel, int threads, size_t smem, int &slots, int &sms) {
+	slots = cache.slots.load();
+	sms = cache.sms.load();
+	if (slots) return cudaSuccess;
+	int dev = 0, occ = 0;
+	cudaError_t e;
+	if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+	if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+	if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, threads, smem)) != cudaSuccess) return e;
+	slots = sms * (occ > 0 ? occ : 1);
+	cache.sms.store(sms); // before slots: a thread that sees slots != 0 also sees sms
+	cache.slots.store(slots);
+	return cudaSuccess;
+}
+
 template <int FMT, int K, int G, int NB, int WPC, bool PRE>
 static cudaError_t launch_st_one(const FeParams &p_in, int forced_L, cudaStream_t s) {
 	constexpr int GG = G <= (1 << (K + 2)) ? G : (1 << (K + 2)); // K = 3: a super-step is 32 samples
@@ -356,18 +374,10 @@ static cudaError_t launch_st_one(const FeParams &p_in, int forced_L, cudaStream_
 	const size_t smem = (size_t)WPC * NB * 32 * StFmt<FMT, GG>::SLOT;
 	cudaError_t e = cudaFuncSetAttribute(k_frontend_st<FMT, K, GG, NB, WPC, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); // per device
 	if (e != cudaSuccess) return e;
-	static std::atomic<int> slots_cache{0}, sms_cache{0}; // SMs x resident CTAs of this instantiation (all devices of a box are alike)
-	int slots = slots_cache.load(std::memory_order_relaxed);
-	if (!slots) {
-		int dev = 0, sms = 0, occ = 0;
-		if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
-		if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
-		if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_frontend_st<FMT, K, GG, NB, WPC, PRE>, WPC * 32, smem)) != cudaSuccess) return e;
-		slots = sms * (occ > 0 ? occ : 1);
-		slots_cache.store(slots, std::memory_order_relaxed);
-		sms_cache.store(sms, std::memory_order_relaxed);
-	}
-	if (p_in.st_cap > 0) slots = std::min(slots, sms_cache.load(std::memory_order_relaxed) * p_in.st_cap);
+	static CtaSlots cache;
+	int slots = 0, sms = 0;
+	if ((e = cta_slots(cache, k_frontend_st<FMT, K, GG, NB, WPC, PRE>, WPC * 32, smem, slots, sms)) != cudaSuccess) return e;
+	if (p_in.st_cap > 0) slots = std::min(slots, sms * p_in.st_cap);
 	FeParams p = p_in;
 	if (p.N % SS || p.P % SS) return cudaErrorNotSupported; // the caller falls back to the tiled kernel
 	if ((unsigned long long)p.st_B * (unsigned long long)p.in_stride * StFmt<FMT, GG>::BPS >= (1ull << 36)) return cudaErrorNotSupported; // 32-bit lane offsets (16-byte units)
@@ -378,16 +388,16 @@ static cudaError_t launch_st_one(const FeParams &p_in, int forced_L, cudaStream_
 	k_frontend_st<FMT, K, GG, NB, WPC, PRE><<<ctas, WPC * 32, smem, s>>>(p);
 	return cudaGetLastError();
 }
-// ring depth x warps per CTA: CF32 (128-byte lane chunks) has the shapes {4 or 6 chunks, 1 warp} and {8 chunks, 4 warps}, one
-// translation unit each; the integer formats (32/64-byte lane chunks) always run one-warp CTAs with 8 chunks
+// One launch shape (chunk length G, ring depth NB, warps per CTA WPC) of one format, for every K it is instantiated for:
+// 3 .. 7 CIC stages (768 kS/s .. 12288 kS/s), or 3 .. 5 in front of DSP::Upsample (pre).  Any other K: cudaErrorNotSupported.
 template <int FMT, int G, int NB, int WPC>
 cudaError_t launch_frontend_stream_shape(const FeParams &p, int k, bool pre, int forced_L, cudaStream_t s) {
 	if (pre) {
-		switch (k) { // CIC stages in front of DSP::Upsample
+		switch (k) {
 		case 3: return launch_st_one<FMT, 3, G, NB, WPC, true>(p, forced_L, s);
 		case 4: return launch_st_one<FMT, 4, G, NB, WPC, true>(p, forced_L, s);
 		case 5: return launch_st_one<FMT, 5, G, NB, WPC, true>(p, forced_L, s);
-		default: return cudaErrorInvalidValue;
+		default: return cudaErrorNotSupported;
 		}
 	}
 	switch (k) {
@@ -396,8 +406,13 @@ cudaError_t launch_frontend_stream_shape(const FeParams &p, int k, bool pre, int
 	case 5: return launch_st_one<FMT, 5, G, NB, WPC, false>(p, forced_L, s);
 	case 6: return launch_st_one<FMT, 6, G, NB, WPC, false>(p, forced_L, s);
 	case 7: return launch_st_one<FMT, 7, G, NB, WPC, false>(p, forced_L, s);
-	default: return cudaErrorInvalidValue;
+	default: return cudaErrorNotSupported;
 	}
 }
+// The shapes that exist, each compiled by its own translation unit only (fe_stream_f0e.cu .. fe_stream_f3.cu)
+extern template cudaError_t launch_frontend_stream_shape<0, 32, 3, 4>(const FeParams &, int, bool, int, cudaStream_t);
+extern template cudaError_t launch_frontend_stream_shape<1, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
+extern template cudaError_t launch_frontend_stream_shape<2, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
+extern template cudaError_t launch_frontend_stream_shape<3, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
 
 } // namespace aisgpu

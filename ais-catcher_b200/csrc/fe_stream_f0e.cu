@@ -1,4 +1,4 @@
-// fe_stream_f0e.cu -- streaming front end: CF32, 32-sample chunks, ring of 3, four-warp CTAs (104 KB: two CTAs per SM, or room for back-end CTAs).
+// fe_stream_f0e.cu -- streaming front end: CF32, 32-sample chunks, ring of 3, four-warp CTAs (104 KB: room for back-end CTAs beside it).
 #include "fe_stream.cuh"
 
 namespace aisgpu {

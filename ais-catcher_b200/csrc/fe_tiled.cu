@@ -87,7 +87,7 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, unsig
 				 : "memory");
 }
 
-// One CTA of NW warps owns (segment, stream) and walks [seg_start - P, seg_end) in tiles of p.tile input samples,
+// One CTA of NW = 4 warps owns (segment, stream) and walks [seg_start - P, seg_end) in tiles of p.tile input samples,
 // starting from zero history: after P >= h_k samples every stage's history is exact, so only 48 kHz outputs that
 // belong to [seg_start, seg_end) are written.  Thread 0 keeps a two-deep ring of bulk async copies (input tile + its
 // Rotate phasors) in flight; all threads then run the stages of the tile back to back out of the CTA's shared-memory
@@ -95,11 +95,7 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, unsig
 // resident warp -- what capped the one-warp version at 6 warps per SM -- drops NW-fold; the deeper (shorter) stages
 // simply occupy fewer warps.  After the barrier that ends a stage, three threads move the last HIST inputs of that
 // stage to the front of the array the next tile will read (the reference's h0..h4 / h1,h2 carried state).
-template <int NW>
-__device__ __forceinline__ void fe_sync() {
-	if (NW == 1) __syncwarp();
-	else __syncthreads();
-}
+constexpr int NW = 4;
 
 // History for the next tile: dst[-HIST .. 0) = src[n - HIST .. n) for a group of stage arrays, n = len >> shift (even;
 // when n < HIST part of the old history moves up -- one warp instruction loads all entries before any is stored).
@@ -115,7 +111,7 @@ __device__ __forceinline__ void fe_carry_group(float2 *__restrict__ sm, const Fe
 	}
 }
 
-template <int FMT, int NW, int K, bool PRE = false>
+template <int FMT, int K, bool PRE = false>
 __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 	constexpr int NT = NW * 32;
 	extern __shared__ __align__(16) float2 sm[];
@@ -153,7 +149,7 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 		else { d.src = d.dst = off_wb; d.shift = K + 1; }
 		cdesc[par][a] = d;
 	}
-	fe_sync<NW>();
+	__syncthreads();
 
 	auto issue = [&](int t) {
 		const int rel = t * p.tile;
@@ -196,7 +192,7 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 				else fe_load_pair<FMT>(p.in, ibase + i, x, y);
 				*reinterpret_cast<float4 *>(sm + off_in + i) = make_float4(x.x, x.y, y.x, y.y);
 			}
-			fe_sync<NW>();
+			__syncthreads();
 		}
 		mbar_wait(&mbar[b], (unsigned)((t >> 1) & 1));
 		// The deeper stages only have work for one or two warps.  Warp w of every CTA sits on scheduler w % 4, so a fixed
@@ -212,7 +208,7 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 			const int n_out = len >> (l + 1);
 			const int vt = FE_VT();
 			for (int j0 = vt * 5; j0 < n_out; j0 += 5 * NT) ds2_run<5>(sm, src, dst, j0);
-			fe_sync<NW>();
+			__syncthreads();
 			if (l == 0 && !PRE) fe_carry_group(sm, cdesc[b], K + 3, 2, p.tile, tid); // wa, wb of the previous (always full) tile; its FilterCIC5 pass is two barriers back
 			src = dst;
 		}
@@ -222,9 +218,9 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 			const int vt_o = FE_VT();
 			for (int i = vt_o; i < nK; i += NT)
 				if (iK + i >= firstK) o[i] = sm[src + i];
-			fe_sync<NW>();
+			__syncthreads();
 			fe_carry_group(sm, cdesc[b], 0, K + 1, len, tid);
-			fe_sync<NW>();
+			__syncthreads();
 			continue;
 		}
 		// ---- FilterComplex3Tap + Rotate at 96 kHz ----
@@ -244,18 +240,18 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 			sm[off_up + i] = make_float2(__fsub_rn(RR, II), __fadd_rn(IR, RI));
 			sm[off_dn + i] = make_float2(__fadd_rn(RR, II), __fsub_rn(IR, RI));
 		}
-		fe_sync<NW>();
+		__syncthreads();
 		if (K == 0) fe_carry_group(sm, cdesc[b], K + 3, 2, p.tile, tid);
 		// ---- per channel Downsample2CIC5 96k -> 48k ----
 		const int n48 = n96 >> 1;
 		const int runs = (n48 + 4) / 5;
-		if (K == 0) fe_sync<NW>(); // the wa/wb history move above reads what this pass overwrites
+		if (K == 0) __syncthreads(); // the wa/wb history move above reads what this pass overwrites
 		const int vt_c = FE_VT();
 		for (int r = vt_c; r < 2 * runs; r += NT) {
 			const int ch = r >= runs;
 			ds2_run<5>(sm, ch ? off_dn : off_up, ch ? off_wb : off_wa, (ch ? r - runs : r) * 5);
 		}
-		fe_sync<NW>();
+		__syncthreads();
 		// every stage that reads the input ring, the level arrays, up and dn has run: move their histories
 		fe_carry_group(sm, cdesc[b], 0, K + 3, len, tid);
 		// ---- per channel FilterCIC5 at 48k, straight to HBM ----
@@ -268,16 +264,16 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 				fcic_run<5>(sm, ch ? off_wb : off_wa, Cg + (ch ? p.c_stride : 0) + m_rel, (ch ? r - runs : r) * 5, m_lo, n48);
 			}
 		}
-		fe_sync<NW>();
+		__syncthreads();
 	}
 }
 
 // ---- launch entry point ----
 template <int FMT, int K, bool PRE>
 static cudaError_t launch_tiled_one(const FeParams &p, dim3 grid, size_t smem, cudaStream_t s) {
-	cudaError_t e = cudaFuncSetAttribute(k_frontend<FMT, 4, K, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+	cudaError_t e = cudaFuncSetAttribute(k_frontend<FMT, K, PRE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
 	if (e != cudaSuccess) return e;
-	k_frontend<FMT, 4, K, PRE><<<grid, 128, smem, s>>>(p);
+	k_frontend<FMT, K, PRE><<<grid, NW * 32, smem, s>>>(p);
 	return cudaGetLastError();
 }
 template <int FMT>

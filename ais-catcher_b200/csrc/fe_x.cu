@@ -131,17 +131,9 @@ cudaError_t launch_x_one(FeParams p, int forced_L, cudaStream_t s) {
 	constexpr int G = XFmt<FMT>::G;
 	constexpr size_t smem = (size_t)X_NB * 32 * XFmt<FMT>::F::SLOT;
 	if (p.N % G || p.P % G || p.N <= 0) return cudaErrorInvalidValue;
-	static std::atomic<int> slots_cache{0}; // SMs x resident CTAs of this instantiation (all devices of a box are alike)
-	int slots = slots_cache.load(std::memory_order_relaxed);
-	if (!slots) {
-		int dev = 0, sms = 0, occ = 0;
-		cudaError_t e;
-		if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
-		if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
-		if ((e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_frontend_x<FMT, K>, 32, smem)) != cudaSuccess) return e;
-		slots = sms * (occ > 0 ? occ : 1);
-		slots_cache.store(slots, std::memory_order_relaxed);
-	}
+	static CtaSlots cache;
+	int slots = 0, sms = 0;
+	if (const cudaError_t e = cta_slots(cache, k_frontend_x<FMT, K>, 32, smem, slots, sms)) return e;
 	const int nss = p.N / G, warm = p.P / G;
 	// sub-segments of at least four warm-ups when the block allows it, else one lane per stream
 	if (!st_plan(p.st_B, nss, warm, 1, slots, 4, forced_L, p.st_L, p.st_q, p.st_r)) {

@@ -36,7 +36,7 @@ struct FeParams {
 	int off_up, off_dn, off_wa, off_wb;
 	int st_L, st_q, st_r, st_B; // streaming kernel: lanes per stream, super-steps per lane (the last st_r lanes of a stream take st_q + 1), streams
 	int st_first;           // 1 in the first block of a stream (the integer front end's virtual history, see fe_stream.cuh)
-	int st_ring, st_cap;    // CF32 launch shape: chunks in the staging ring (3 or 5; 0 = 5) and resident CTAs per SM the lane planner counts on (0 = what fits)
+	int st_cap;             // resident CTAs per SM the lane planner counts on (0 = what fits)
 	int smem_f2;          // total float2
 	float2 *D0;           // PRE mode (decimation in front of DSP::Upsample): level-K samples, [B][d0_stride], sample i at d0_off + i
 	long long d0_stride;
@@ -184,10 +184,8 @@ cudaError_t set_taps_bh28_3(const float *taps26);
 // fe_tiled.cu
 cudaError_t launch_frontend_tiled(const FeParams &p, int fmt, int k, bool pre, dim3 grid, size_t smem, cudaStream_t s);
 // fe_stream_f*.cu: the launcher picks the lanes per stream (st_plan in fe_stream.cuh) unless forced_L > 0
-cudaError_t launch_frontend_stream(const FeParams &p, int fmt, int k, bool pre, int forced_L, cudaStream_t s); // cudaErrorNotSupported: block too short for this kernel
+cudaError_t launch_frontend_stream(const FeParams &p, int fmt, int k, bool pre, int forced_L, cudaStream_t s); // cudaErrorNotSupported: no shape for k, or the block does not fit the kernel
 cudaError_t launch_frontend_stream_fpds(const FeParams &p, int forced_L, cudaStream_t s); // fe_stream_fp.cu: CU8, integer CIC stages, 1536K
-template <int FMT, int G, int NB, int WPC>
-cudaError_t launch_frontend_stream_shape(const FeParams &p, int k, bool pre, int forced_L, cudaStream_t s);
 // fe_x.cu: single-channel mode, k = 0 .. 2 CIC stages, one Cbuf row per stream; p.N and p.P multiples of frontend_x_granule(fmt)
 cudaError_t launch_frontend_x(const FeParams &p, int fmt, int k, int forced_L, cudaStream_t s);
 int frontend_x_granule(int fmt);
@@ -198,8 +196,7 @@ cudaError_t launch_frontend_disc(const FeParams &p, int fmt, cudaStream_t s);
 cudaError_t cgf_init(const float *taps17, const float2 *omega256);
 cudaError_t launch_cgf_estimate(const float2 *Cbuf, long long c_stride, int c_begin, int nblk, int total_blocks, const float2 *omega, int wide, int *stepidx, cudaStream_t s);
 cudaError_t launch_cgf_fused(const float2 *Cbuf, long long c_stride, int c_begin, const int *stepidx, const float2 *steptab, float2 *rot_state, int nblk, int rows,
-                             const float2 *hist_old, float2 *hist_new, float2 *Ebuf, long long e_stride, int e_off, float2 *tap_cgf, long long tap_stride, int rows_per_cta,
-                             cudaStream_t s);
+                             const float2 *hist_old, float2 *hist_new, float2 *Ebuf, long long e_stride, int e_off, float2 *tap_cgf, long long tap_stride, cudaStream_t s);
 // be_v2.cu
 cudaError_t v2_init(const float *taps17, const float *taps37, const float2 *omega256);
 cudaError_t launch_v2_engine(const float2 *Cbuf, long long c_stride, int c_begin, int nproc, int rows, V2State *st, DecState *dec, uint32_t *dec_data, FrameRec *ring,
