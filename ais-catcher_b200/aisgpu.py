@@ -21,7 +21,8 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_last_frontend_ms", "aisgpu_frontend_times", "aisgpu_last_launches", "aisgpu_last_error", "aisgpu_destroy",
            "aisgpu_validate", "aisgpu_build_nmea", "aisgpu_chunk_granule", "aisgpu_join", "aisgpu_submit_v", "aisgpu_submit_async",
            "aisgpu_poll_upto", "aisgpu_nccl_unique_id", "aisgpu_comm_init", "aisgpu_allreduce_counts",
-           "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch"]
+           "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
+           "aisgpu_check_attach"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW = 0, -1, -2, -3, -4, -5
 
@@ -112,6 +113,9 @@ def load():
     lib.aisgpu_chunk_granule.argtypes = [C.POINTER(Config)]
     if hasattr(lib, "aisgpu_check_device_batch"):  # absent from libraries built before the placement rule (AISGPU_LIB)
         lib.aisgpu_check_device_batch.argtypes = [C.POINTER(Config), C.c_void_p, C.c_int64]
+    if hasattr(lib, "aisgpu_attach"):  # absent from libraries built before engine groups (AISGPU_LIB)
+        lib.aisgpu_attach.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(C.c_void_p)]
+        lib.aisgpu_check_attach.argtypes = [C.POINTER(Config), C.POINTER(Config)]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -219,23 +223,50 @@ def nccl_unique_id():
     return buf.raw
 
 
+def make_config(model=MODEL_DEFAULT, sample_rate=1536000, fmt=FMT_CF32, n_streams=1, max_chunk=131072, ps_ema=True, afc_wide=True,
+                droop=True, own_mmsi=-1, device=0, taps=False, max_frames=0, tag_mode=3, host_staging=True, dsk=False, fp_ds=False,
+                channel_mode=MODE_AB, channels="AB", dd_train=0.75, dd_weight=0.86):
+    """aisgpu_config from Engine's keyword arguments (the library's defaults for everything else)."""
+    cfg = Config()
+    load().aisgpu_default_config(C.byref(cfg))
+    cfg.model, cfg.sample_rate, cfg.format = model, sample_rate, fmt
+    cfg.n_streams, cfg.max_chunk_samples = n_streams, max_chunk
+    cfg.ps_ema, cfg.afc_wide, cfg.droop = int(ps_ema), int(afc_wide), int(droop)
+    cfg.own_mmsi, cfg.device, cfg.enable_taps, cfg.max_frames, cfg.tag_mode = own_mmsi, device, int(taps), max_frames, tag_mode
+    cfg.host_staging, cfg.dsk, cfg.fp_ds = int(host_staging), int(dsk), int(fp_ds)
+    cfg.dd_train, cfg.dd_weight = dd_train, dd_weight
+    cfg.channel_mode = channel_mode
+    cfg.channel_a, cfg.channel_b = channels[0].encode(), channels[1].encode()  # CH1 / CH2 of buildModel
+    return cfg
+
+
+# what a group member may set for itself (aisgpu_attach); every other field is the leader's
+MEMBER_KEYS = ("model", "ps_ema", "afc_wide", "dd_train", "dd_weight", "channels", "own_mmsi", "taps", "max_frames", "tag_mode")
+
+
+def check_attach(leader, member):
+    """aisgpu_check_attach (no GPU needed): leader and member are dicts of Engine keyword arguments.  Raises with the reason (the
+    first front-end field that differs) if the member may not join the leader's group."""
+    lib = load()
+    rc = lib.aisgpu_check_attach(C.byref(make_config(**leader)), C.byref(make_config(**member)))
+    if rc:
+        raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode()))
+
+
 class Engine:
     """One batch engine == one AIS::Model instance per stream of the batch (reference Source/DSP/Model.h:76-126)."""
 
     def __init__(self, model=MODEL_DEFAULT, sample_rate=1536000, fmt=FMT_CF32, n_streams=1, max_chunk=131072,
                  ps_ema=True, afc_wide=True, droop=True, own_mmsi=-1, device=0, taps=False, max_frames=0, tag_mode=3, host_staging=True,
-                 dsk=False, fp_ds=False, channel_mode=MODE_AB, channels="AB"):
+                 dsk=False, fp_ds=False, channel_mode=MODE_AB, channels="AB", dd_train=0.75, dd_weight=0.86):
         self.lib = load()
-        cfg = Config()
-        self.lib.aisgpu_default_config(C.byref(cfg))
-        cfg.model, cfg.sample_rate, cfg.format = model, sample_rate, fmt
-        cfg.n_streams, cfg.max_chunk_samples = n_streams, max_chunk
-        cfg.ps_ema, cfg.afc_wide, cfg.droop = int(ps_ema), int(afc_wide), int(droop)
-        cfg.own_mmsi, cfg.device, cfg.enable_taps, cfg.max_frames, cfg.tag_mode = own_mmsi, device, int(taps), max_frames, tag_mode
-        cfg.host_staging, cfg.dsk, cfg.fp_ds = int(host_staging), int(dsk), int(fp_ds)
-        cfg.channel_mode = channel_mode
-        cfg.channel_a, cfg.channel_b = channels[0].encode(), channels[1].encode()  # CH1 / CH2 of buildModel
+        self.kwargs = dict(model=model, sample_rate=sample_rate, fmt=fmt, n_streams=n_streams, max_chunk=max_chunk, ps_ema=ps_ema,
+                           afc_wide=afc_wide, droop=droop, own_mmsi=own_mmsi, device=device, taps=taps, max_frames=max_frames,
+                           tag_mode=tag_mode, host_staging=host_staging, dsk=dsk, fp_ds=fp_ds, channel_mode=channel_mode,
+                           channels=channels, dd_train=dd_train, dd_weight=dd_weight)
+        cfg = make_config(**self.kwargs)
         self.cfg = cfg
+        self.leader = None
         self.h = C.c_void_p()
         rc = self.lib.aisgpu_create(C.byref(cfg), C.byref(self.h))
         if rc:
@@ -243,6 +274,27 @@ class Engine:
         self.n_streams = n_streams
         self.fmt = fmt
         self.overflows = 0  # polls that reported AISGPU_EOVERFLOW (frames were dropped; the survivors were delivered)
+
+    def attach(self, **member):
+        """aisgpu_attach: a new engine of this one's group with its own back end (keyword arguments: MEMBER_KEYS, the rest is this
+        engine's).  It is fed by this engine's submits; its own submit methods raise.  Attach before the first submit, and close
+        the members before the leader."""
+        bad = sorted(set(member) - set(MEMBER_KEYS))
+        if bad:
+            raise TypeError("attach() sets only the back end (%s); the front end is the leader's: %s" % (", ".join(MEMBER_KEYS), ", ".join(bad)))
+        if len(member.get("channels", "AB")) != 2:
+            raise ValueError("channels must be two letters (CH1, CH2), got %r" % (member["channels"],))
+        kw = dict(self.kwargs, **member)
+        cfg = make_config(**kw)
+        h = C.c_void_p()
+        rc = self.lib.aisgpu_attach(self.h, C.byref(cfg), C.byref(h))
+        if rc:
+            raise AisGpuError("aisgpu_attach rc=%d: %s" % (rc, self.lib.aisgpu_last_error(None).decode()))
+        m = Engine.__new__(Engine)
+        m.lib, m.kwargs, m.cfg, m.h = self.lib, kw, cfg, h
+        m.leader = self  # keeps the leader alive while the member exists
+        m.n_streams, m.fmt, m.overflows = self.n_streams, self.fmt, 0
+        return m
 
     def _chk(self, rc):
         if rc == EOVERFLOW:

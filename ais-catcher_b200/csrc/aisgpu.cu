@@ -231,6 +231,13 @@ struct aisgpu_handle {
 	// NCCL (resolved at run time): communicator of the job's ranks, device scratch of the counter all-reduce
 	void *nccl_lib = nullptr, *nccl_comm = nullptr;
 	unsigned long long *d_counts = nullptr;
+	// Engine groups (aisgpu_attach): a member has no front end of its own; every inner submit of its leader copies the leader's new
+	// 48 kHz rows into the member's own Cbuf ring (k_c_fanout on the leader's fe_stream, then ev_fan) and runs the member's back end.
+	aisgpu_config given;                    // the caller's config as passed to aisgpu_create / aisgpu_attach (the rule compares these)
+	bool member = false;                    // created by aisgpu_attach (stays set when the leader is destroyed)
+	aisgpu_handle *leader = nullptr;        // member: its leader while both exist
+	std::vector<aisgpu_handle *> members;   // leader: in attach order
+	cudaEvent_t ev_fan = nullptr;           // leader: recorded behind k_c_fanout, waited on by every member's back end
 };
 
 namespace {
@@ -739,7 +746,12 @@ int enqueue_rot_table(aisgpu_handle *h, long long c, int n96) {
 	return 0;
 }
 
-// One Receive() of the front end proper: N samples per stream (a whole reference block) -> frames.
+int fan_out(aisgpu_handle *h, int cb, int n48);
+int backend_begin(aisgpu_handle *h, cudaEvent_t ready, int N, int n48);
+int backend_step(aisgpu_handle *h, float2 *Ccur, float2 *Cnext, int n48);
+
+// One Receive() of the front end proper: N samples per stream (a whole reference block) -> frames, for the engine and the members
+// of its group.
 int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	const int q = (h->xmode || h->disc) ? X_GRANULE : 1 << (h->k + 2);
 	if (N <= 0 || N > h->inner_max || (N % q) != 0) {
@@ -787,13 +799,53 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 		h->last_launches++;
 	}
 	CU(cudaEventRecord(h->ev_fe_done[cb], h->fe_stream));
+	if (!h->members.empty())
+		if (int rc = fan_out(h, cb, n48)) return rc;
+	if (int rc = backend_begin(h, h->ev_fe_done[cb], N, n48)) return rc;
+	if (int rc = backend_step(h, Ccur, Cnext, n48)) return rc;
+	for (aisgpu_handle *m : h->members) {
+		int rc = backend_begin(m, h->ev_fan, N, n48);
+		if (!rc) rc = backend_step(m, m->d_C2[cb], m->d_C2[(cb + 1) % aisgpu_handle::NC], n48);
+		if (rc) {
+			h->err = m->err;
+			return rc;
+		}
+	}
+	return 0;
+}
+
+// Engine groups: the leader's new rows [HC, HC + n48) of Cbuf[cb] into every member's Cbuf[cb], on the leader's fe_stream behind its
+// front end.  A member's Cbuf[cb] was last read by its back end of submit c-3.
+int fan_out(aisgpu_handle *h, int cb, int n48) {
+	float2 *dst[GROUP_MAX - 1];
+	int nd = 0;
+	for (aisgpu_handle *m : h->members) {
+		if (m->be_recorded[cb]) CU(cudaStreamWaitEvent(h->fe_stream, m->ev_be_done[cb], 0));
+		dst[nd++] = m->d_C2[cb];
+	}
+	CU(launch_c_fanout(h->d_C2[cb], dst, nd, h->c_stride, HC, n48, h->rows, h->fe_stream));
+	CU(cudaEventRecord(h->ev_fan, h->fe_stream));
+	h->last_launches++;
+	return 0;
+}
+
+// The back end of one inner submit starts when its 48 kHz rows are ready: the engine's own front end, or its leader's fan-out.
+int backend_begin(aisgpu_handle *h, cudaEvent_t ready, int N, int n48) {
+	h->c_last = (int)(h->chunk % aisgpu_handle::NC);
 	h->pb = (int)(h->chunk & 1);
 	h->bs = h->be_streams[h->pb];
-	CU(cudaStreamWaitEvent(h->bs, h->ev_fe_done[cb], 0));
+	CU(cudaStreamWaitEvent(h->bs, ready, 0));
 	h->last_n = N;
 	h->last_n48 = n48;
 	h->last_nE = 0;
 	h->last_nsym = 0;
+	return 0;
+}
+
+// Everything behind the 48 kHz rows of one inner submit: n48 new samples per row at [HC, HC + n48) of Ccur; what the chain carries
+// into the next submit goes in front of HC in Cnext.
+int backend_step(aisgpu_handle *h, float2 *Ccur, float2 *Cnext, int n48) {
+	const int cb = (int)(h->chunk % aisgpu_handle::NC);
 	// ---- back end (stage-pipelined over consecutive submits, see aisgpu_handle::be_streams) ----
 	if (h->cfg.model == AISGPU_MODEL_V2) {
 		// Engine::Receive (V2Engine.cpp:379-395): a block is decoded once the NEXT block is complete (it is the estimator's
@@ -992,6 +1044,10 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 	if (int rc = check_outer(h, N)) return rc;
 	h->last_launches = 0;
 	h->msg_chunk = (long long)h->counters[3];
+	for (aisgpu_handle *m : h->members) {
+		m->last_launches = 0;
+		m->msg_chunk = h->msg_chunk;
+	}
 	const int B = h->cfg.n_streams;
 	int rc = 0;
 	h->pre_tap0 = h->s_produced;
@@ -1107,6 +1163,14 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 	h->pre_tap1 = h->s_produced;
 	h->pre2_tap1 = h->s2_produced;
 	if (int rc2 = mark_ticket(h, (long long)h->counters[3])) return rc2;
+	for (aisgpu_handle *m : h->members) {
+		if (int rc2 = mark_ticket(m, (long long)h->counters[3])) {
+			h->err = m->err;
+			return rc2;
+		}
+		m->counters[2] += (uint64_t)N;
+		m->counters[3] += 1;
+	}
 	h->counters[2] += (uint64_t)N;
 	h->counters[3] += 1;
 	return 0;
@@ -1316,6 +1380,7 @@ const char *aisgpu_last_error(aisgpu_handle *h) { return h ? h->err.c_str() : g_
 // hooks for the host-only units of the library (host_internal.h)
 const aisgpu_config *aisgpu_internal_config(aisgpu_handle *h) { return &h->cfg; }
 void aisgpu_internal_set_error(aisgpu_handle *h, const char *msg) { h->err = msg; }
+int aisgpu_internal_grouped(aisgpu_handle *h) { return h->member || !h->members.empty(); }
 
 static int create_impl(aisgpu_handle *h) {
 	const aisgpu_config &c = h->cfg;
@@ -1401,7 +1466,8 @@ static int create_impl(aisgpu_handle *h) {
 	h->inner_max = h->pre == 1 ? (maxN >> h->kA) : (h->pre >= 2 ? h->blk : maxN);
 	h->max_n48 = h->inner_max >> ((h->xmode || h->disc) ? k : k + 1);
 	h->seq.assign(B, 0);
-	if (h->pre) { // resampler pre-stage: raw-format history, decimated stream, schedule tables, ring of reference blocks
+	// a group member (aisgpu_attach) has no front end: no pre-stage, warm-up tails, Rotate tables or input staging
+	if (h->pre && !h->member) { // resampler pre-stage: raw-format history, decimated stream, schedule tables, ring of reference blocks
 		const int tl = h->pre == 2 ? 32 : h->PA;
 		for (int i = 0; i < 2; i++) {
 			if (int rc = dalloc(h, &h->d_ptail[i], (size_t)B * tl * h->obps)) return rc;
@@ -1437,14 +1503,14 @@ static int create_impl(aisgpu_handle *h) {
 		if (int rc = dalloc(h, &h->d_S, (size_t)B * h->s_stride)) return rc;
 	}
 	for (int i = 0; i < 2; i++) {
-		if (h->P) {
+		if (h->P && !h->member) {
 			if (int rc = dalloc(h, &h->d_tail[i], (size_t)B * h->P * h->bps)) return rc;
 			if (h->in_fmt == AISGPU_FMT_CU8 && !h->fp_ds) // the reference's zero initial filter state is byte value 128 in CU8 (0 for the unbiased integer pipeline)
 				CU(cudaMemsetAsync(h->d_tail[i], 0x80, (size_t)B * h->P * h->bps, h->stream));
 		}
 		if (int rc = dalloc(h, &h->d_fir_hist[i], (size_t)h->rows * 16)) return rc;
 	}
-	if (!h->xmode && !h->disc) {
+	if (!h->xmode && !h->disc && !h->member) {
 		for (int i = 0; i < 3; i++)
 			if (int rc = dalloc(h, &h->d_rot[i], (size_t)h->P96 + (h->inner_max >> k) + 8)) return rc;
 		if (int rc = dalloc(h, &h->d_rot_state, 4)) return rc;
@@ -1583,7 +1649,7 @@ static int create_impl(aisgpu_handle *h) {
 	memset(h->pin_head, 0, aisgpu_handle::NT * sizeof(unsigned long long));
 	for (int i = 0; i < aisgpu_handle::NT; i++) CU(cudaEventCreateWithFlags(&h->ev_ticket[i], cudaEventDisableTiming));
 	CU(cudaEventCreateWithFlags(&h->ev_mark, cudaEventDisableTiming));
-	if (h->pre == 1 || h->pre == 3) {
+	if ((h->pre == 1 || h->pre == 3) && !h->member) {
 		h->us_cap = h->us_ratio * (maxN >> h->kA) + 8; // Upsample emits at most ceil(bucket / rate) samples per input
 		for (int i = 0; i < 2; i++) {
 			if (cudaMallocHost((void **)&h->pin_us_src[i], (size_t)h->us_cap * sizeof(int)) != cudaSuccess ||
@@ -1595,7 +1661,7 @@ static int create_impl(aisgpu_handle *h) {
 			CU(cudaEventCreateWithFlags(&h->ev_us[i], cudaEventDisableTiming));
 		}
 	}
-	if (c.host_staging) // the H2D staging buffers of aisgpu_submit / _v / _async (otherwise allocated by the first host submit)
+	if (c.host_staging && !h->member) // the H2D staging buffers of aisgpu_submit / _v / _async (otherwise allocated by the first host submit)
 		for (int i = 0; i < 2; i++)
 			if (int rc = dalloc(h, &h->d_in[i], (size_t)B * maxN * h->obps)) return rc;
 	memset(&h->fe, 0, sizeof(h->fe));
@@ -1621,6 +1687,7 @@ int aisgpu_create(const aisgpu_config *cfg, aisgpu_handle **out) {
 	}
 	aisgpu_handle *h = new aisgpu_handle();
 	h->cfg = c;
+	h->given = c;
 	int rc = create_impl(h);
 	if (rc) {
 		g_create_error = h->err;
@@ -1633,8 +1700,16 @@ int aisgpu_create(const aisgpu_config *cfg, aisgpu_handle **out) {
 }
 
 // a CUDA failure (or an internal inconsistency) inside a submit leaves carried state half-advanced: poison the handle
+// (a group's submit advances every member's state too: the whole group is poisoned)
 static int poison(aisgpu_handle *h, int rc) {
-	if (rc != 0 && rc != AISGPU_EINVAL && !h->poisoned) h->poisoned = rc;
+	if (rc != 0 && rc != AISGPU_EINVAL && !h->poisoned) {
+		h->poisoned = rc;
+		for (aisgpu_handle *m : h->members)
+			if (!m->poisoned) {
+				m->poisoned = rc;
+				m->err = h->err;
+			}
+	}
 	return rc;
 }
 #define ENTER(h)                                  \
@@ -1644,8 +1719,16 @@ static int poison(aisgpu_handle *h, int rc) {
 		CU(cudaSetDevice((h)->cfg.device));       \
 	} while (0)
 
+// a group member is fed by its leader's submits only
+static int refuse_member(aisgpu_handle *h) {
+	if (!h->member) return 0;
+	h->err = "this engine is a member of a group: submit to the group's leader";
+	return AISGPU_EINVAL;
+}
+
 int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stride_samples, int n_samples) {
 	ENTER(h);
+	if (int rc = refuse_member(h)) return rc;
 	if (!dev_samples) return AISGPU_EINVAL;
 	if (int rc = check_placement(h, dev_samples, stride_samples)) return rc;
 	if (stride_samples < n_samples) {
@@ -1693,18 +1776,21 @@ static int submit_host(aisgpu_handle *h, const void *host_samples, const void *c
 
 int aisgpu_submit(aisgpu_handle *h, const void *host_samples, int n_samples) {
 	ENTER(h);
+	if (int rc = refuse_member(h)) return rc;
 	if (!host_samples) return AISGPU_EINVAL;
 	return poison(h, submit_host(h, host_samples, nullptr, n_samples, true, nullptr));
 }
 
 int aisgpu_submit_v(aisgpu_handle *h, const void *const *stream_ptrs, int n_samples) {
 	ENTER(h);
+	if (int rc = refuse_member(h)) return rc;
 	if (!stream_ptrs) return AISGPU_EINVAL;
 	return poison(h, submit_host(h, nullptr, stream_ptrs, n_samples, true, nullptr));
 }
 
 int aisgpu_submit_async(aisgpu_handle *h, const void *host_samples, int n_samples, int64_t *ticket) {
 	ENTER(h);
+	if (int rc = refuse_member(h)) return rc;
 	if (!host_samples) return AISGPU_EINVAL;
 	return poison(h, submit_host(h, host_samples, nullptr, n_samples, false, ticket));
 }
@@ -1714,6 +1800,11 @@ int aisgpu_sync(aisgpu_handle *h) {
 	CU(cudaStreamSynchronize(h->copy_stream));
 	CU(cudaStreamSynchronize(h->fe_stream));
 	if (int rc = sync_backend(h)) return rc;
+	for (aisgpu_handle *m : h->members)
+		if (int rc = sync_backend(m)) {
+			h->err = m->err;
+			return rc;
+		}
 	return 0;
 }
 
@@ -1749,6 +1840,10 @@ int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, si
 	}
 	if (h->disc && tap == AISGPU_TAP_ROT) {
 		h->err = "the FM discriminator model has no Rotate";
+		return AISGPU_EINVAL;
+	}
+	if (h->member && (tap == AISGPU_TAP_ROT || tap == AISGPU_TAP_PRE || tap == AISGPU_TAP_PRE2)) {
+		h->err = "a group member has no front end: read the front-end taps from the group's leader";
 		return AISGPU_EINVAL;
 	}
 	const int row = row_of(h, stream, channel & 1);
@@ -1947,6 +2042,11 @@ int aisgpu_join(aisgpu_handle *h) {
 		CU(cudaEventRecord(h->ev_join, h->be_streams[1]));
 		CU(cudaStreamWaitEvent(h->stream, h->ev_join, 0));
 	}
+	for (aisgpu_handle *m : h->members) // the event is captured by each wait, so one serves every back-end stream of the group
+		for (int i = 0; i < (m->be_streams[1] != m->be_streams[0] ? 2 : 1); i++) {
+			CU(cudaEventRecord(h->ev_join, m->be_streams[i]));
+			CU(cudaStreamWaitEvent(h->stream, h->ev_join, 0));
+		}
 	return 0;
 }
 
@@ -2007,6 +2107,86 @@ int aisgpu_check_device_batch(const aisgpu_config *cfg, const void *dev_samples,
 	return rc;
 }
 
+// The rule of aisgpu_attach on two caller configs: every field the front end reads is equal, and neither engine is the
+// FM-discriminator input model (its front end is the I/Q split, not the CIC chain the others share).
+static int check_attach_cfg(const aisgpu_config &L, const aisgpu_config &M, std::string &err) {
+	const struct {
+		const char *name;
+		long long a, b;
+	} fields[] = { { "sample_rate", L.sample_rate, M.sample_rate }, { "format", L.format, M.format }, { "n_streams", L.n_streams, M.n_streams },
+				   { "max_chunk_samples", L.max_chunk_samples, M.max_chunk_samples }, { "channel_mode", L.channel_mode, M.channel_mode },
+				   { "droop", L.droop, M.droop }, { "dsk", L.dsk, M.dsk }, { "fp_ds", L.fp_ds, M.fp_ds }, { "device", L.device, M.device } };
+	for (const auto &f : fields)
+		if (f.a != f.b) {
+			err = std::string("aisgpu_attach: ") + f.name + " differs from the leader's (a group shares the leader's front end)";
+			return AISGPU_EINVAL;
+		}
+	if (L.model == AISGPU_MODEL_DISCRIMINATOR || M.model == AISGPU_MODEL_DISCRIMINATOR) {
+		err = std::string("aisgpu_attach: the FM discriminator model cannot be in a group (as the ") +
+			  (L.model == AISGPU_MODEL_DISCRIMINATOR ? "leader)" : "member)");
+		return AISGPU_EINVAL;
+	}
+	return 0;
+}
+
+int aisgpu_check_attach(const aisgpu_config *leader, const aisgpu_config *member) {
+	aisgpu_config l, m;
+	if (!copy_config(leader, &l) || !copy_config(member, &m)) {
+		g_create_error = "aisgpu_check_attach: null argument or struct_size mismatch";
+		return AISGPU_EINVAL;
+	}
+	return check_attach_cfg(l, m, g_create_error);
+}
+
+int aisgpu_attach(aisgpu_handle *leader, const aisgpu_config *cfg, aisgpu_handle **out) {
+	aisgpu_config c;
+	if (!leader || !out || !copy_config(cfg, &c)) {
+		g_create_error = "aisgpu_attach: null argument or struct_size mismatch";
+		return AISGPU_EINVAL;
+	}
+	*out = nullptr;
+	if (leader->poisoned) {
+		g_create_error = "aisgpu_attach: the leader has failed: " + leader->err;
+		return leader->poisoned;
+	}
+	if (int rc = check_attach_cfg(leader->given, c, g_create_error)) return rc;
+	if (leader->member) {
+		g_create_error = "aisgpu_attach: a member cannot lead a group";
+		return AISGPU_EINVAL;
+	}
+	if (leader->counters[3] != 0) {
+		g_create_error = "aisgpu_attach: the leader has already been submitted to (attach every member before the first submit)";
+		return AISGPU_EINVAL;
+	}
+	if ((int)leader->members.size() + 1 >= GROUP_MAX) {
+		g_create_error = "aisgpu_attach: a group holds at most 8 engines";
+		return AISGPU_EINVAL;
+	}
+	if (cudaSetDevice(leader->cfg.device) != cudaSuccess || (!leader->ev_fan && cudaEventCreateWithFlags(&leader->ev_fan, cudaEventDisableTiming) != cudaSuccess)) {
+		(void)cudaGetLastError();
+		g_create_error = "aisgpu_attach: CUDA event creation failed";
+		return AISGPU_ECUDA;
+	}
+	aisgpu_handle *h = new aisgpu_handle();
+	h->cfg = c;
+	h->given = c;
+	h->member = true;
+	int rc = create_impl(h);
+	if (!rc && (h->rows != leader->rows || h->c_stride != leader->c_stride || h->inner_max != leader->inner_max)) {
+		h->err = "internal: a member's 48 kHz rows differ from its leader's";
+		rc = AISGPU_EINVAL;
+	}
+	if (rc) {
+		g_create_error = h->err;
+		aisgpu_destroy(h);
+		return rc;
+	}
+	h->leader = leader;
+	leader->members.push_back(h);
+	*out = h;
+	return 0;
+}
+
 int aisgpu_validate(const uint8_t *data, int nbits) {
 	if (!data || nbits < 0) return 0;
 	return msg_validate(data, nbits) ? 1 : 0;
@@ -2020,7 +2200,22 @@ int aisgpu_build_nmea(aisgpu_msg *m, int own_mmsi, int *seq) {
 
 void aisgpu_destroy(aisgpu_handle *h) {
 	if (!h) return;
+	if (h->leader) { // detach: the leader's fe_stream may still be writing this member's rows
+		cudaSetDevice(h->leader->cfg.device);
+		cudaStreamSynchronize(h->leader->fe_stream);
+		auto &v = h->leader->members;
+		v.erase(std::remove(v.begin(), v.end(), h), v.end());
+		h->leader = nullptr;
+	}
 	if (h->fe_stream) cudaStreamSynchronize(h->fe_stream);
+	for (aisgpu_handle *m : h->members) { // their back ends were waiting on this engine's front end
+		cudaStreamSynchronize(m->be_streams[0]);
+		if (m->be_streams[1] != m->be_streams[0]) cudaStreamSynchronize(m->be_streams[1]);
+		m->leader = nullptr;
+		if (!m->poisoned) m->poisoned = AISGPU_EINVAL;
+		m->err = "the group's leader was destroyed (destroy the members first)";
+	}
+	if (h->ev_fan) cudaEventDestroy(h->ev_fan);
 	if (h->stream) cudaStreamSynchronize(h->stream);
 	if (h->be_streams[1] && h->be_streams[1] != h->stream) { cudaStreamSynchronize(h->be_streams[1]); cudaStreamDestroy(h->be_streams[1]); }
 	for (int st = 0; st < aisgpu_handle::NSTAGE; st++)

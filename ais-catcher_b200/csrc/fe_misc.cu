@@ -1,4 +1,6 @@
 // fe_misc.cu -- small front-end kernels: Rotate phasor table, Upsample, DownsampleKFilter, history carries.
+#include <algorithm>
+
 #include "exact.cuh"
 #include "params.h"
 #include "fe_common.cuh"
@@ -115,6 +117,26 @@ __global__ void k_carry2(const T *__restrict__ src, T *__restrict__ dst, long lo
 	for (int i = threadIdx.x; i < cnt; i += blockDim.x) drow[i] = srow[i];
 }
 
+// Engine groups: one read of the leader's new 48 kHz rows, written to every member's own ring (aisgpu.cu, fan_out).  16-byte loads
+// and stores: rows, offset and length are whole float4s.  The member pointers are unrolled so that they stay in the parameter bank.
+struct FanoutArgs {
+	const float4 *src;
+	float4 *dst[GROUP_MAX - 1];
+	long long stride4;
+	int off4, n4, rows, nd;
+};
+__global__ void __launch_bounds__(256) k_c_fanout(const FanoutArgs a) {
+	for (int r = blockIdx.y; r < a.rows; r += gridDim.y) {
+		const long long row = (long long)r * a.stride4 + a.off4;
+		for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < a.n4; j += gridDim.x * blockDim.x) {
+			const float4 v = a.src[row + j];
+#pragma unroll
+			for (int m = 0; m < GROUP_MAX - 1; m++)
+				if (m < a.nd) a.dst[m][row + j] = v;
+		}
+	}
+}
+
 __global__ void k_d0_carry(float2 *__restrict__ D0, long long d0_stride, int d0_off, int L, int rows) {
 	const int r = blockIdx.x * blockDim.x + threadIdx.x;
 	if (r < rows) D0[(long long)r * d0_stride + d0_off - 1] = D0[(long long)r * d0_stride + d0_off + L - 1]; // Upsample::a = b
@@ -165,6 +187,21 @@ cudaError_t launch_carry_f2(float2 *buf, long long stride, int src_begin, int ds
 }
 cudaError_t launch_carry2_f2(const float2 *src, float2 *dst, long long stride, int src_begin, int dst_begin, int cnt, int rows, cudaStream_t s) {
 	k_carry2<float2><<<rows, 128, 0, s>>>(src, dst, stride, src_begin, dst_begin, cnt);
+	return cudaGetLastError();
+}
+cudaError_t launch_c_fanout(const float2 *src, float2 *const *dst, int nd, long long stride, int off, int n, int rows, cudaStream_t s) {
+	if (nd < 1 || nd > GROUP_MAX - 1 || (stride | off | n) & 1) return cudaErrorInvalidValue;
+	FanoutArgs a;
+	a.src = reinterpret_cast<const float4 *>(src);
+	for (int m = 0; m < GROUP_MAX - 1; m++) a.dst[m] = m < nd ? reinterpret_cast<float4 *>(dst[m]) : nullptr;
+	a.stride4 = stride / 2;
+	a.off4 = off / 2;
+	a.n4 = n / 2;
+	a.rows = rows;
+	a.nd = nd;
+	if (a.n4 == 0) return cudaSuccess;
+	const dim3 grid((a.n4 + 255) / 256, std::min(rows, 65535));
+	k_c_fanout<<<grid, 256, 0, s>>>(a);
 	return cudaGetLastError();
 }
 cudaError_t set_taps_bh28_3(const float *taps26) { return cudaMemcpyToSymbol(c_taps_bh28_3, taps26, DSK_T * sizeof(float)); }

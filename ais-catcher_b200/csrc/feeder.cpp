@@ -45,6 +45,10 @@ void read_block(std::vector<Source> &src, int s0, int s1, unsigned char *dst, si
 
 extern "C" int aisgpu_feed_files(aisgpu_handle *h, const char *const *paths, int n_samples, aisgpu_msg_fn fn, void *user, uint64_t *n_blocks) {
 	if (!h) return AISGPU_EINVAL;
+	if (aisgpu_internal_grouped(h)) {
+		aisgpu_internal_set_error(h, "aisgpu_feed_files: not available for an engine group (aisgpu_attach)");
+		return AISGPU_EINVAL;
+	}
 	const aisgpu_config *cfg = aisgpu_internal_config(h);
 	if (!paths || n_samples <= 0 || n_samples > cfg->max_chunk_samples) {
 		aisgpu_internal_set_error(h, "aisgpu_feed_files: bad argument");

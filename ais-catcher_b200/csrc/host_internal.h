@@ -4,4 +4,5 @@
 extern "C" {
 const aisgpu_config *aisgpu_internal_config(aisgpu_handle *h);
 void aisgpu_internal_set_error(aisgpu_handle *h, const char *msg);
+int aisgpu_internal_grouped(aisgpu_handle *h); // 1 for a member of an engine group or a leader with members
 }

@@ -273,7 +273,36 @@ int aisgpu_msg_binary(const aisgpu_msg *m, const aisgpu_tag *tag, int crc, uint8
 typedef void (*aisgpu_msg_fn)(const aisgpu_msg *msgs, int n, void *user);
 int aisgpu_feed_files(aisgpu_handle *h, const char *const *paths, int n_samples, aisgpu_msg_fn fn, void *user, uint64_t *n_blocks);
 
-const char *aisgpu_last_error(aisgpu_handle *h); /* h may be NULL: error of the last failed aisgpu_create */
+/* ---- Engine groups: several models on one front end (the reference's repeated -m, Receiver.cpp:126-244) ----
+ *
+ * Makes *out a member of leader's group: an engine with a back end of its own (cfg->model with its own ps_ema, afc_wide, dd_train,
+ * dd_weight, channel_a/b, station, own_mmsi, tag_mode, enable_taps, max_frames) that is fed with the 48 kHz channel rows of the
+ * leader's front end instead of running the front end again.  Call it before the leader's first submit.  AISGPU_EINVAL (reason in
+ * aisgpu_last_error(NULL)) when aisgpu_check_attach refuses the pair, when the leader has been submitted to, when leader is itself a
+ * member, or when the group would exceed 8 engines.
+ *
+ * A member behaves exactly like a standalone engine of its own config that received the leader's submits:
+ *   - aisgpu_poll, aisgpu_poll_upto (with the leader's tickets), aisgpu_counters and aisgpu_tap act on the member's own frame ring
+ *     and state: emission order, msg.chunk, sequence ids, AISGPU_EOVERFLOW and the counters are the standalone engine's; counters[2]
+ *     and [3] follow the leader's submits;
+ *   - only the leader is submitted to (aisgpu_submit, _v, _async, _device); one leader submit runs every member's back end.
+ *     aisgpu_submit* on a member, and aisgpu_feed_files on a leader with members, return AISGPU_EINVAL;
+ *   - aisgpu_sync(leader) and aisgpu_join(leader) cover the whole group (events on the leader's stream time the group);
+ *   - a member has no front end: AISGPU_TAP_ROT, _PRE and _PRE2 are AISGPU_EINVAL, aisgpu_last_frontend_ms() is -1 and
+ *     aisgpu_frontend_times() gives n = 0;
+ *   - a CUDA failure in a group submit poisons every engine of the group;
+ *   - destroying a member detaches it (the leader's frames do not change); destroying a leader that still has members poisons
+ *     them, so destroy the members first.
+ * One thread drives a whole group, as for a single handle. */
+int aisgpu_attach(aisgpu_handle *leader, const aisgpu_config *cfg, aisgpu_handle **out);
+
+/* The compatibility rule of aisgpu_attach without touching the GPU: 0, or AISGPU_EINVAL with the reason (naming the first field that
+ * differs) in aisgpu_last_error(NULL).  Every front-end field must be equal -- sample_rate, format, n_streams, max_chunk_samples,
+ * channel_mode, droop, dsk, fp_ds, device -- and neither config may be AISGPU_MODEL_DISCRIMINATOR.  struct_size as for
+ * aisgpu_create. */
+int aisgpu_check_attach(const aisgpu_config *leader, const aisgpu_config *member);
+
+const char *aisgpu_last_error(aisgpu_handle *h); /* h may be NULL: error of the last failed aisgpu_create / aisgpu_attach */
 
 /* == ~Model */
 void aisgpu_destroy(aisgpu_handle *h);

@@ -89,4 +89,13 @@ with tempfile.TemporaryDirectory() as d:  # file feeder, CU8, ragged lengths, FP
     msgs, nb = eng.feed_files(paths, N)
     print("feeder blocks", nb, "messages", len(msgs))
     eng.close()
+eng = aisgpu.Engine(model=aisgpu.MODEL_DEFAULT, sample_rate=fs, n_streams=B, max_chunk=N)  # engine group: one front end, three back ends
+mem = [eng.attach(model=aisgpu.MODEL_STANDARD), eng.attach(model=aisgpu.MODEL_V2)]
+for c in range(3):
+    eng.submit(np.stack([x[c * N:(c + 1) * N] for x in xs]), N)
+    if c == 1:
+        mem.pop(0).close()  # a member destroyed mid-run
+print("group messages", len(eng.poll()), len(mem[0].poll()))
+mem[0].close()
+eng.close()
 print("sanitizer workload done")
