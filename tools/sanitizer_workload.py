@@ -29,6 +29,18 @@ for fmt, nodd in ((aisgpu.FMT_CF32, 64 * 257), (aisgpu.FMT_CU8, 64 * 131)):  # b
         eng.submit(np.stack([aissynth.to_cu8(r) for r in blk]) if fmt == aisgpu.FMT_CU8 else blk, nodd)
     print("odd block", nodd, "fmt", fmt, "messages", len(eng.poll()))
     eng.close()
+import edge_signals  # silence, exact-zero gaps and clipped traffic beside ordinary rows, CF32 and CU8
+for model in (aisgpu.MODEL_STANDARD, aisgpu.MODEL_DEFAULT, aisgpu.MODEL_V2):
+    for fmt in (aisgpu.FMT_CF32, aisgpu.FMT_CU8):
+        rows = [edge_signals.make(k, fs, N * 4, 800 + i, fmt, submit=N, granule=64)[0] for i, k in enumerate(("silence", "gaps", "clipped"))]
+        rows.insert(1, mode_x_util.to_raw(xs[0], fmt)[0])
+        rows.insert(3, mode_x_util.to_raw(xs[1], fmt)[0])
+        per = 1 if fmt == aisgpu.FMT_CF32 else 2
+        eng = aisgpu.Engine(model=model, sample_rate=fs, fmt=fmt, n_streams=5, max_chunk=N)
+        for c in range(4):
+            eng.submit(np.stack([r[c * N * per:(c + 1) * N * per] for r in rows]), N)
+        print("edge rows model", model, "fmt", fmt, "messages", len(eng.poll()))
+        eng.close()
 eng = aisgpu.Engine(model=aisgpu.MODEL_DEFAULT, sample_rate=6000000, n_streams=2, max_chunk=32768)  # resampler pre-stage
 x6 = np.stack([aissynth.random_stream(6000000, 32768 * 3, 400 + s)[0] for s in range(2)])
 for c in range(3):
