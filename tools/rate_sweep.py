@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """GPU: step throughput for the other BASELINE.json configs (rate sweep, 6 MSPS AirSpy shape, PhaseSearch variants).
-usage: rate_sweep.py fs:B:N:model:ps_ema ...   (synthetic bursts + noise, device-resident input, R=3 chunks cycled)"""
+usage: rate_sweep.py fs:B:N:model:ps_ema[:dsk] ...   (synthetic bursts + noise, device-resident input, R=3 chunks cycled; dsk: -go DSK on)"""
 import json
 import os
 import sys
@@ -16,7 +16,7 @@ import aissynth
 dev = torch.device("cuda", 0)
 peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 3350.0  # H100 SXM data sheet, not measured
 for spec in sys.argv[1:]:
-    fs, B, N, model, ps_ema = [int(v) for v in spec.split(":")]
+    fs, B, N, model, ps_ema, dsk = ([int(v) for v in spec.split(":")] + [0])[:6]
     R, U = 3, 8
     uniq = np.stack([aissynth.random_stream(fs, N * R, 2000 + u)[0] for u in range(U)])
     ud = torch.from_numpy(uniq.view(np.float32)).to(dev).view(U, N * R, 2)
@@ -28,7 +28,7 @@ for spec in sys.argv[1:]:
     for r in range(R):
         x[r] += torch.randn_like(x[r]) * 0.005
     torch.cuda.synchronize()
-    eng = aisgpu.Engine(model=model, sample_rate=fs, n_streams=B, max_chunk=N, ps_ema=bool(ps_ema), max_frames=1 << 21)
+    eng = aisgpu.Engine(model=model, sample_rate=fs, n_streams=B, max_chunk=N, ps_ema=bool(ps_ema), dsk=bool(dsk), max_frames=1 << 21)
     for i in range(3):
         eng.submit_device(x[i % R].data_ptr(), N, N)
     eng.sync()
@@ -51,7 +51,7 @@ for spec in sys.argv[1:]:
         iso.append(eng.last_frontend_ms())
     eng.poll()
     gbs = B * N * 8 / ms / 1e6
-    print(json.dumps({"fs": fs, "B": B, "N": N, "model": model, "ps_ema": ps_ema, "ms_per_step": round(ms, 4), "GSps": round(B * N / ms / 1e6, 1),
+    print(json.dumps({"fs": fs, "B": B, "N": N, "model": model, "ps_ema": ps_ema, "dsk": dsk, "ms_per_step": round(ms, 4), "GSps": round(B * N / ms / 1e6, 1),
                       "input_GBps": round(gbs, 1), "frac_of_hbm_peak": round(gbs / peak, 3), "last_frontend_launch_ms": round(min(iso), 4),
                       "msgs_per_step": nm // K}), flush=True)
     eng.close()
