@@ -1271,11 +1271,10 @@ cudaError_t launch_decode10(int rpw, const K3Params &p, cudaStream_t s) {
 cudaError_t launch_decode(int model, int decoder, int rpw, const K3Params &p, cudaStream_t s) {
 	return model == 2 ? launch_decode_model<2>(decoder, rpw, p, s) : launch_decode_model<0>(decoder, rpw, p, s);
 }
-cudaError_t launch_base(const float *Ef, long long e_stride, int e_begin, int n, int rows, PllState *pll, DecState *dec, uint32_t *dec_data, FrameRec *ring,
-						unsigned long long *ring_head, unsigned long long ring_limit, int ring_cap, int chunk, int blk, float *tap_dec, int *tap_cnt,
-						cudaStream_t s) {
-	k_base<<<(rows + K3_THREADS - 1) / K3_THREADS, K3_THREADS, 0, s>>>(Ef, e_stride, e_begin, n, rows, pll, dec, dec_data, ring, ring_head, ring_limit, ring_cap, chunk,
-																		  blk, tap_dec, tap_cnt);
+cudaError_t launch_base(const float *Ef, long long e_stride, int e_begin, int n, int rows, PllState *pll, DecState *dec, uint32_t *dec_data,
+						const FrameOut &out, float *tap_dec, int *tap_cnt, cudaStream_t s) {
+	k_base<<<(rows + K3_THREADS - 1) / K3_THREADS, K3_THREADS, 0, s>>>(Ef, e_stride, e_begin, n, rows, pll, dec, dec_data, out.ring, out.ring_head, out.ring_limit,
+																		  out.ring_cap, out.chunk, out.blk, tap_dec, tap_cnt);
 	return cudaGetLastError();
 }
 

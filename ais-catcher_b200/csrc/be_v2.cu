@@ -386,12 +386,13 @@ cudaError_t v2_init(const float *taps17, const float *taps37, const float2 *omeg
 	if (e == cudaSuccess) e = cudaFuncSetAttribute(k_v2_engine, cudaFuncAttributeMaxDynamicSharedMemorySize, V2_WARPS * V2_WARP_BYTES);
 	return e;
 }
-cudaError_t launch_v2_engine(const float2 *Cbuf, long long c_stride, int c_begin, int nproc, int rows, V2State *st, DecState *dec, uint32_t *dec_data, FrameRec *ring,
-							 unsigned long long *ring_head, unsigned long long ring_limit, int ring_cap, int chunk, int blk, int mode_level, const float2 *omega_g,
-							 float w_train, float w_track, float2 *tap_fc, float2 *tap_coh, float *tap_fmf, long long tap_stride, cudaStream_t s) {
+cudaError_t launch_v2_engine(const float2 *Cbuf, long long c_stride, int c_begin, int nproc, int rows, V2State *st, DecState *dec, uint32_t *dec_data,
+							 const FrameOut &out, const float2 *omega_g, float w_train, float w_track, float2 *tap_fc, float2 *tap_coh, float *tap_fmf,
+							 long long tap_stride, cudaStream_t s) {
 	V2Params p;
 	p.Cbuf = Cbuf; p.c_stride = c_stride; p.c_begin = c_begin; p.nproc = nproc; p.rows = rows; p.st = st; p.dec = dec; p.dec_data = dec_data;
-	p.ring = ring; p.ring_head = ring_head; p.ring_limit = ring_limit; p.ring_cap = ring_cap; p.chunk = chunk; p.blk = blk; p.mode_level = mode_level;
+	p.ring = out.ring; p.ring_head = out.ring_head; p.ring_limit = out.ring_limit; p.ring_cap = out.ring_cap; p.chunk = out.chunk; p.blk = out.blk;
+	p.mode_level = out.mode_level;
 	p.omega_g = omega_g; p.w_train = w_train; p.w_track = w_track; p.tap_fc = tap_fc; p.tap_coh = tap_coh; p.tap_fmf = tap_fmf; p.tap_stride = tap_stride;
 	k_v2_engine<<<(rows + V2_WARPS - 1) / V2_WARPS, V2_WARPS * 32, V2_WARPS * V2_WARP_BYTES, s>>>(p);
 	return cudaGetLastError();

@@ -100,6 +100,17 @@ struct FrameRec {
 	int blk;              // ordinal of the front-end block (several per submit behind a resampler)
 };
 
+// Host side: the frame ring of one decoder launch, as the launchers take it (the kernels receive the fields one by one)
+struct FrameOut {
+	FrameRec *ring;
+	unsigned long long *ring_head; // frames emitted since the engine was created (tickets); slot = ticket % ring_cap
+	unsigned long long ring_limit; // tickets below this may be written: frames drained by the host at launch time + ring_cap
+	int ring_cap;
+	int chunk;                     // ordinal of the caller's submit
+	int blk;                       // ordinal of the front-end block
+	int mode_level;                // tag_mode & 1: frames carry the signal level
+};
+
 
 struct K3Params {
 	int ps_ema;
@@ -203,9 +214,9 @@ cudaError_t launch_cgf_fused(const float2 *Cbuf, long long c_stride, int c_begin
                              const float2 *hist_old, float2 *hist_new, float2 *Ebuf, long long e_stride, int e_off, float2 *tap_cgf, long long tap_stride, cudaStream_t s);
 // be_v2.cu
 cudaError_t v2_init(const float *taps17, const float *taps37, const float2 *omega256);
-cudaError_t launch_v2_engine(const float2 *Cbuf, long long c_stride, int c_begin, int nproc, int rows, V2State *st, DecState *dec, uint32_t *dec_data, FrameRec *ring,
-                             unsigned long long *ring_head, unsigned long long ring_limit, int ring_cap, int chunk, int blk, int mode_level, const float2 *omega_g,
-                             float w_train, float w_track, float2 *tap_fc, float2 *tap_coh, float *tap_fmf, long long tap_stride, cudaStream_t s);
+cudaError_t launch_v2_engine(const float2 *Cbuf, long long c_stride, int c_begin, int nproc, int rows, V2State *st, DecState *dec, uint32_t *dec_data,
+                             const FrameOut &out, const float2 *omega_g, float w_train, float w_track, float2 *tap_fc, float2 *tap_coh, float *tap_fmf,
+                             long long tap_stride, cudaStream_t s);
 // be_fm.cu
 cudaError_t fm_init(const float *taps37);
 cudaError_t launch_fm_fir5(const Fm5Params &p, int rows, cudaStream_t s);
@@ -214,8 +225,8 @@ cudaError_t sym_init(const float *ps_cos8, const float *ps_sin8, const uint32_t 
 cudaError_t launch_phase_search(const K3Params &p, cudaStream_t s);
 cudaError_t launch_decode(int model, int decoder, int rpw, const K3Params &p, cudaStream_t s);
 cudaError_t launch_decode10(int rpw, const K3Params &p, cudaStream_t s);
-cudaError_t launch_base(const float *Ef, long long e_stride, int e_begin, int n, int rows, PllState *pll, DecState *dec, uint32_t *dec_data, FrameRec *ring,
-                        unsigned long long *ring_head, unsigned long long ring_limit, int ring_cap, int chunk, int blk, float *tap_dec, int *tap_cnt,
-                        cudaStream_t s);
+// out.mode_level is not read: k_base always sums the level (its sample levels are 0)
+cudaError_t launch_base(const float *Ef, long long e_stride, int e_begin, int n, int rows, PllState *pll, DecState *dec, uint32_t *dec_data,
+                        const FrameOut &out, float *tap_dec, int *tap_cnt, cudaStream_t s);
 
 } // namespace aisgpu
