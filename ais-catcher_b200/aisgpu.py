@@ -22,9 +22,9 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_validate", "aisgpu_build_nmea", "aisgpu_chunk_granule", "aisgpu_join", "aisgpu_submit_v", "aisgpu_submit_async",
            "aisgpu_poll_upto", "aisgpu_nccl_unique_id", "aisgpu_comm_init", "aisgpu_allreduce_counts",
            "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
-           "aisgpu_check_attach"]
+           "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close"]
 
-OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW = 0, -1, -2, -3, -4, -5
+OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 
 
 class Config(C.Structure):
@@ -116,6 +116,9 @@ def load():
     if hasattr(lib, "aisgpu_attach"):  # absent from libraries built before engine groups (AISGPU_LIB)
         lib.aisgpu_attach.argtypes = [C.c_void_p, C.POINTER(Config), C.POINTER(C.c_void_p)]
         lib.aisgpu_check_attach.argtypes = [C.POINTER(Config), C.POINTER(Config)]
+    if hasattr(lib, "aisgpu_dump_open"):  # absent from libraries built before the channel dump (AISGPU_LIB)
+        lib.aisgpu_dump_open.argtypes = [C.c_void_p, C.POINTER(C.c_char_p)]
+        lib.aisgpu_dump_close.argtypes = [C.c_void_p]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -435,6 +438,23 @@ class Engine:
 
     def last_launches(self):
         return int(self.lib.aisgpu_last_launches(self.h))
+
+    def dump_open(self, prefixes):
+        """aisgpu_dump_open (-go DUMP): prefixes is one entry per stream, a path prefix (str or os.PathLike) or None for a stream
+        that is not dumped.  Stream s goes to <prefix>_A.wav and <prefix>_B.wav.  Open before the first submit."""
+        prefixes = list(prefixes)
+        if len(prefixes) != self.n_streams:
+            raise ValueError("dump_open: %d prefixes for %d streams" % (len(prefixes), self.n_streams))
+        arr = (C.c_char_p * len(prefixes))(*[None if p is None else os.fsencode(p) for p in prefixes])
+        rc = self.lib.aisgpu_dump_open(self.h, arr)
+        if rc:
+            raise AisGpuError("rc=%d: %s" % (rc, self.lib.aisgpu_last_error(self.h).decode()))
+
+    def dump_close(self):
+        """aisgpu_dump_close: writes what is pending, patches the WAV headers and closes the files."""
+        rc = self.lib.aisgpu_dump_close(self.h)
+        if rc:
+            raise AisGpuError("rc=%d: %s" % (rc, self.lib.aisgpu_last_error(self.h).decode()))
 
     def close(self):
         if self.h:

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/aisgpu.h"
+#include "dump.h"
 #include "params.h"
 
 using namespace aisgpu;
@@ -267,6 +268,25 @@ struct aisgpu_handle {
 	aisgpu_handle *leader = nullptr;        // member: its leader while both exist
 	std::vector<aisgpu_handle *> members;   // leader: in attach order
 	cudaEvent_t ev_fan = nullptr;           // leader: recorded behind k_c_fanout, waited on by every member's back end
+	// The 48 kHz channel dump (aisgpu_dump_open).  Each inner submit's new rows are gathered (k_c_fanout on fe_stream, behind
+	// ev_fe_done) into columns [dump_off, dump_off + n48) of the submit's device slot [rows][dump_n]; after the last pass dump_stream
+	// copies the slot into its pinned twin and records ev_dump.  The caller's thread writes the pinned slot to the files (dump_write).
+	// Slot s is reused by submit j only after the host has written its previous contents, which also means that the previous copy
+	// out of d_dump[s] has finished.  Nothing of this is allocated or launched while no dump has been opened.
+	static const int ND = 3;
+	aisgpu::ChannelDump *dump = nullptr;
+	cudaStream_t dump_stream = nullptr;
+	float2 *d_dump[3] = { nullptr, nullptr, nullptr }, *pin_dump[3] = { nullptr, nullptr, nullptr };
+	cudaEvent_t ev_dump[3] = { nullptr, nullptr, nullptr }, ev_export = nullptr;
+	long long dump_cap = 0;  // samples per row a slot holds: the most one submit can yield
+	long long dump_next = 0; // submits that have filled a slot; slot dump_next % ND is the next one
+	struct DumpPending {
+		long long ticket, n;
+		int slot;
+	};
+	std::deque<DumpPending> dump_pending; // slots copied or being copied, not yet written, in submit order
+	int dump_slot = -1;                   // the submit being enqueued: its slot (-1: no export), row length and columns exported so far
+	long long dump_n = 0, dump_off = 0;
 	// everything dalloc, halloc and new_event created: aisgpu_destroy releases these (the streams are destroyed one by one)
 	std::vector<void *> dev_mem, host_mem;
 	std::vector<cudaEvent_t> events;
@@ -669,6 +689,7 @@ int enqueue_rot_table(aisgpu_handle *h, long long c, int n96) {
 }
 
 int fan_out(aisgpu_handle *h, int cb, int n48);
+int dump_export(aisgpu_handle *h, int cb, int n48);
 int backend_begin(aisgpu_handle *h, cudaEvent_t ready, int N, int n48);
 int backend_step(aisgpu_handle *h, float2 *Ccur, float2 *Cnext, int n48);
 
@@ -723,6 +744,8 @@ int submit_common(aisgpu_handle *h, const void *dev_in, long long stride, int N)
 	CU(cudaEventRecord(h->ev_fe_done[cb], h->fe_stream));
 	if (!h->members.empty())
 		if (int rc = fan_out(h, cb, n48)) return rc;
+	if (h->dump_slot >= 0)
+		if (int rc = dump_export(h, cb, n48)) return rc;
 	if (int rc = backend_begin(h, h->ev_fe_done[cb], N, n48)) return rc;
 	if (int rc = backend_step(h, Ccur, Cnext, n48)) return rc;
 	for (aisgpu_handle *m : h->members) {
@@ -745,9 +768,85 @@ int fan_out(aisgpu_handle *h, int cb, int n48) {
 		if (m->be_recorded[cb]) CU(cudaStreamWaitEvent(h->fe_stream, m->ev_be_done[cb], 0));
 		dst[nd++] = m->d_C2[cb];
 	}
-	CU(launch_c_fanout(h->d_C2[cb], dst, nd, h->c_stride, HC, n48, h->rows, h->fe_stream));
+	CU(launch_c_fanout(h->d_C2[cb], h->c_stride, HC, dst, nd, h->c_stride, HC, n48, h->rows, h->fe_stream));
 	CU(cudaEventRecord(h->ev_fan, h->fe_stream));
 	h->last_launches++;
+	return 0;
+}
+
+// ---- the channel dump (aisgpu_dump_open) ----
+
+// Before the first pass of a submit that yields n 48 kHz samples per row: pick its slot.  The host has already written the slot's
+// previous contents (dump_reclaim); the front-end stream still waits for the copy out of it, which has finished by then.
+int dump_begin(aisgpu_handle *h, long long n) {
+	h->dump_slot = -1;
+	if (!h->dump || n == 0) return 0;
+	const int s = (int)(h->dump_next % aisgpu_handle::ND);
+	if (n > h->dump_cap || h->dump_pending.size() >= (size_t)aisgpu_handle::ND) {
+		h->err = "internal: channel dump slot overrun";
+		return AISGPU_ECUDA;
+	}
+	if (h->dump_next >= aisgpu_handle::ND) CU(cudaStreamWaitEvent(h->fe_stream, h->ev_dump[s], 0));
+	h->dump_slot = s;
+	h->dump_n = n;
+	h->dump_off = 0;
+	return 0;
+}
+
+// One inner submit: its rows [HC, HC + n48) of Cbuf[cb] into columns [dump_off, dump_off + n48) of the slot, on fe_stream behind
+// ev_fe_done[cb] (no back end waits for it) and behind a leader's fan-out (no member waits for it either).
+int dump_export(aisgpu_handle *h, int cb, int n48) {
+	if (h->dump_off + n48 > h->dump_n) {
+		h->err = "internal: channel dump export overrun";
+		return AISGPU_ECUDA;
+	}
+	float2 *dst = h->d_dump[h->dump_slot];
+	CU(launch_c_fanout(h->d_C2[cb], h->c_stride, HC, &dst, 1, h->dump_n, (int)h->dump_off, n48, h->rows, h->fe_stream));
+	h->dump_off += n48;
+	h->last_launches++;
+	return 0;
+}
+
+// After the last pass: one copy of the whole slot into its pinned twin on dump_stream.
+int dump_end(aisgpu_handle *h, long long ticket) {
+	const int s = h->dump_slot;
+	if (s < 0) return 0;
+	h->dump_slot = -1;
+	if (h->dump_off != h->dump_n) {
+		h->err = "internal: channel dump rows missing";
+		return AISGPU_ECUDA;
+	}
+	CU(cudaEventRecord(h->ev_export, h->fe_stream));
+	CU(cudaStreamWaitEvent(h->dump_stream, h->ev_export, 0));
+	CU(cudaMemcpyAsync(h->pin_dump[s], h->d_dump[s], (size_t)h->rows * h->dump_n * sizeof(float2), cudaMemcpyDeviceToHost, h->dump_stream));
+	CU(cudaEventRecord(h->ev_dump[s], h->dump_stream));
+	h->dump_pending.push_back({ ticket, h->dump_n, s });
+	h->dump_next++;
+	return 0;
+}
+
+// Writes the pending slots of the submits up to `ticket` (all of them for ticket < 0) to the files, in submit order, on the caller's
+// thread.  After a file error the rows are dropped (the dump has stopped); the error surfaces at the next submit.
+int dump_write(aisgpu_handle *h, long long ticket) {
+	while (!h->dump_pending.empty() && (ticket < 0 || h->dump_pending.front().ticket <= ticket)) {
+		const aisgpu_handle::DumpPending p = h->dump_pending.front();
+		CU(cudaEventSynchronize(h->ev_dump[p.slot]));
+		h->dump_pending.pop_front();
+		if (h->dump && !h->dump->failed()) h->dump->write(reinterpret_cast<const float *>(h->pin_dump[p.slot]), p.n);
+	}
+	return 0;
+}
+
+// At the entry of every submit, before anything is enqueued: a stopped dump refuses the submit (the reference's StopRequest());
+// otherwise the slot this submit may fill is written out first if it still holds an earlier submit's rows.
+int dump_reclaim(aisgpu_handle *h) {
+	if (!h->dump) return 0;
+	if (h->dump_pending.size() >= (size_t)aisgpu_handle::ND)
+		if (int rc = dump_write(h, h->dump_pending.front().ticket)) return rc;
+	if (h->dump->failed()) {
+		h->err = h->dump->error();
+		return AISGPU_EIO;
+	}
 	return 0;
 }
 
@@ -1258,6 +1357,7 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 		m->msg_chunk = h->msg_chunk;
 	}
 	if (!h->pre_us && !h->pre_dsk) {
+		if (int rc = dump_begin(h, N >> (h->k + 1))) return rc; // a dump is AB only: two 48 kHz rows per stream
 		if (int rc = submit_common(h, dev_in, stride, N)) return rc;
 	}
 	else {
@@ -1279,9 +1379,12 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 			for (PreRing &u = h->us_ring; u.produced - u.consumed >= h->us_blk; u.consumed += h->us_blk)
 				if (int rc = pre_dsk(h, u.d + u.consumed % u.cap, u.stride, h->us_blk)) return rc;
 		// hand every whole reference block of the last ring to the front end proper
-		for (PreRing &r = h->pre_dsk ? h->dsk_ring : h->us_ring; r.produced - r.consumed >= h->blk; r.consumed += h->blk)
+		PreRing &r = h->pre_dsk ? h->dsk_ring : h->us_ring;
+		if (int rc = dump_begin(h, (r.produced - r.consumed) / h->blk * (h->blk >> (h->k + 1)))) return rc;
+		for (; r.produced - r.consumed >= h->blk; r.consumed += h->blk)
 			if (int rc = submit_common(h, r.d + r.consumed % r.cap, r.stride, h->blk)) return rc;
 	}
+	if (int rc = dump_end(h, (long long)h->counters[3])) return rc;
 	if (int rc2 = mark_ticket(h, (long long)h->counters[3])) return rc2;
 	for (aisgpu_handle *m : h->members) {
 		if (int rc2 = mark_ticket(m, (long long)h->counters[3])) {
@@ -1742,6 +1845,13 @@ static int refuse_member(aisgpu_handle *h) {
 	return AISGPU_EINVAL;
 }
 
+// The checks of every submit before anything is enqueued: the length, then the channel dump (a stopped dump refuses the submit with
+// AISGPU_EIO, which does not poison the handle; a slot still holding rows is written out)
+static int submit_gate(aisgpu_handle *h, int n_samples) {
+	if (int rc = check_outer(h, n_samples)) return rc;
+	return dump_reclaim(h);
+}
+
 int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stride_samples, int n_samples) {
 	ENTER(h);
 	if (int rc = refuse_member(h)) return rc;
@@ -1751,7 +1861,7 @@ int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stri
 		h->err = "stride_samples must be >= n_samples";
 		return AISGPU_EINVAL;
 	}
-	if (int rc = check_outer(h, n_samples)) return rc; // all argument checks come before any state is touched
+	if (int rc = submit_gate(h, n_samples)) return rc; // all argument checks come before any state is touched
 	return poison(h, submit_outer(h, dev_samples, stride_samples, n_samples));
 }
 
@@ -1794,6 +1904,7 @@ int aisgpu_submit(aisgpu_handle *h, const void *host_samples, int n_samples) {
 	ENTER(h);
 	if (int rc = refuse_member(h)) return rc;
 	if (!host_samples) return AISGPU_EINVAL;
+	if (int rc = submit_gate(h, n_samples)) return rc;
 	return poison(h, submit_host(h, host_samples, nullptr, n_samples, true, nullptr));
 }
 
@@ -1801,6 +1912,7 @@ int aisgpu_submit_v(aisgpu_handle *h, const void *const *stream_ptrs, int n_samp
 	ENTER(h);
 	if (int rc = refuse_member(h)) return rc;
 	if (!stream_ptrs) return AISGPU_EINVAL;
+	if (int rc = submit_gate(h, n_samples)) return rc;
 	return poison(h, submit_host(h, nullptr, stream_ptrs, n_samples, true, nullptr));
 }
 
@@ -1808,6 +1920,7 @@ int aisgpu_submit_async(aisgpu_handle *h, const void *host_samples, int n_sample
 	ENTER(h);
 	if (int rc = refuse_member(h)) return rc;
 	if (!host_samples) return AISGPU_EINVAL;
+	if (int rc = submit_gate(h, n_samples)) return rc;
 	return poison(h, submit_host(h, host_samples, nullptr, n_samples, false, ticket));
 }
 
@@ -1821,12 +1934,13 @@ int aisgpu_sync(aisgpu_handle *h) {
 			h->err = m->err;
 			return rc;
 		}
-	return 0;
+	return dump_write(h, -1);
 }
 
 int aisgpu_poll_upto(aisgpu_handle *h, int64_t ticket, aisgpu_msg *out, int max, int *n) {
 	if (!n || (max > 0 && !out)) return AISGPU_EINVAL;
 	ENTER(h);
+	if (int rc = dump_write(h, ticket > (int64_t)h->counters[3] - 1 ? -1 : (long long)ticket)) return rc;
 	if (h->out_pos >= h->out_queue.size()) {
 		h->out_queue.clear();
 		h->out_pos = 0;
@@ -2063,6 +2177,10 @@ int aisgpu_join(aisgpu_handle *h) {
 			CU(cudaEventRecord(h->ev_join, m->be_streams[i]));
 			CU(cudaStreamWaitEvent(h->stream, h->ev_join, 0));
 		}
+	if (h->dump_stream) { // the copies of the channel dump
+		CU(cudaEventRecord(h->ev_join, h->dump_stream));
+		CU(cudaStreamWaitEvent(h->stream, h->ev_join, 0));
+	}
 	return 0;
 }
 
@@ -2203,6 +2321,51 @@ int aisgpu_attach(aisgpu_handle *leader, const aisgpu_config *cfg, aisgpu_handle
 	return 0;
 }
 
+static int dump_refuse(aisgpu_handle *h, const char *why) {
+	h->err = std::string("aisgpu_dump_open: ") + why;
+	return AISGPU_EINVAL;
+}
+
+int aisgpu_dump_open(aisgpu_handle *h, const char *const *prefixes) {
+	ENTER(h);
+	if (!prefixes) return dump_refuse(h, "null prefix array");
+	if (h->member) return dump_refuse(h, "a group member has no front end of its own (dump the group's leader)");
+	if (h->cfg.model == AISGPU_MODEL_DISCRIMINATOR) return dump_refuse(h, "the FM-discriminator input model has no 48 kHz channel dump (ModelDiscriminator refuses the key)");
+	if (h->xmode) return dump_refuse(h, "single-channel mode writes no channel dump (the reference wires none in mode X)");
+	if (h->dump) return dump_refuse(h, "a dump is already open");
+	if (h->counters[3] != 0) return dump_refuse(h, "the engine has already been submitted to (open the dump before the first submit)");
+	// the most 48 kHz samples per row one submit can yield: whole blocks of the last pre-stage ring (< one block left over plus what
+	// one submit adds, within the ring's capacity) times a block's samples, or one submit's without a pre-stage
+	const long long nblk = h->pre_dsk ? h->dsk_ring.cap / h->blk : (h->pre_us ? h->us_ratio + 2 : 1);
+	const long long cap = nblk * h->max_n48;
+	if (!h->dump_stream) {
+		CU(cudaStreamCreateWithFlags(&h->dump_stream, cudaStreamNonBlocking));
+		CU(new_event(h, &h->ev_export));
+		for (int i = 0; i < aisgpu_handle::ND; i++) {
+			if (int rc = dalloc(h, &h->d_dump[i], (size_t)h->rows * cap)) return rc;
+			if (int rc = halloc(h, &h->pin_dump[i], (size_t)h->rows * cap)) return rc;
+			CU(new_event(h, &h->ev_dump[i]));
+		}
+		CU(cudaStreamSynchronize(h->stream)); // dalloc clears on h->stream
+		h->dump_cap = cap;
+	}
+	h->dump = new aisgpu::ChannelDump(prefixes, h->cfg.n_streams);
+	return 0;
+}
+
+int aisgpu_dump_close(aisgpu_handle *h) {
+	if (!h) return AISGPU_EINVAL;
+	if (!h->dump) return 0;
+	CU(cudaSetDevice(h->cfg.device));
+	const int rc = h->poisoned ? h->poisoned : dump_write(h, -1); // a poisoned engine's slots are not trusted: close with what was written
+	h->dump_pending.clear();
+	const bool ok = h->dump->close();
+	if (!ok) h->err = h->dump->error();
+	delete h->dump;
+	h->dump = nullptr;
+	return rc ? rc : (ok ? 0 : AISGPU_EIO);
+}
+
 int aisgpu_validate(const uint8_t *data, int nbits) {
 	if (!data || nbits < 0) return 0;
 	return msg_validate(data, nbits) ? 1 : 0;
@@ -2216,6 +2379,7 @@ int aisgpu_build_nmea(aisgpu_msg *m, int own_mmsi, int *seq) {
 
 void aisgpu_destroy(aisgpu_handle *h) {
 	if (!h) return;
+	if (h->dump) aisgpu_dump_close(h);
 	if (h->leader) { // detach: the leader's fe_stream may still be writing this member's rows
 		cudaSetDevice(h->leader->cfg.device);
 		cudaStreamSynchronize(h->leader->fe_stream);
@@ -2239,12 +2403,14 @@ void aisgpu_destroy(aisgpu_handle *h) {
 	}
 	if (h->copy_stream) cudaStreamSynchronize(h->copy_stream);
 	if (h->side_stream) cudaStreamSynchronize(h->side_stream);
+	if (h->dump_stream) cudaStreamSynchronize(h->dump_stream);
 	for (void *p : h->dev_mem) cudaFree(p);
 	for (void *p : h->host_mem) cudaFreeHost(p);
 	for (cudaEvent_t e : h->events) cudaEventDestroy(e);
 	if (h->side_stream) cudaStreamDestroy(h->side_stream);
 	if (h->fe_stream) cudaStreamDestroy(h->fe_stream);
 	if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
+	if (h->dump_stream) cudaStreamDestroy(h->dump_stream);
 	if (h->stream) cudaStreamDestroy(h->stream);
 	delete h;
 }

@@ -117,22 +117,25 @@ __global__ void k_carry2(const T *__restrict__ src, T *__restrict__ dst, long lo
 	for (int i = threadIdx.x; i < cnt; i += blockDim.x) drow[i] = srow[i];
 }
 
-// Engine groups: one read of the leader's new 48 kHz rows, written to every member's own ring (aisgpu.cu, fan_out).  16-byte loads
-// and stores: rows, offset and length are whole float4s.  The member pointers are unrolled so that they stay in the parameter bank.
+// One read of n new 48 kHz samples per row, written to up to GROUP_MAX - 1 destinations at a stride and offset of their own:
+//  - engine groups: the leader's rows into every member's own ring, at the Cbuf stride and HC (aisgpu.cu, fan_out);
+//  - the channel dump: the rows of one inner submit into columns [off, off + n) of the submit's compact export slot (dump_export).
+// 16-byte loads and stores: strides, offsets and length are whole float4s.  The destination pointers are unrolled so that they stay
+// in the parameter bank.
 struct FanoutArgs {
 	const float4 *src;
 	float4 *dst[GROUP_MAX - 1];
-	long long stride4;
-	int off4, n4, rows, nd;
+	long long src_stride4, dst_stride4;
+	int src_off4, dst_off4, n4, rows, nd;
 };
 __global__ void __launch_bounds__(256) k_c_fanout(const FanoutArgs a) {
 	for (int r = blockIdx.y; r < a.rows; r += gridDim.y) {
-		const long long row = (long long)r * a.stride4 + a.off4;
+		const long long srow = (long long)r * a.src_stride4 + a.src_off4, drow = (long long)r * a.dst_stride4 + a.dst_off4;
 		for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < a.n4; j += gridDim.x * blockDim.x) {
-			const float4 v = a.src[row + j];
+			const float4 v = a.src[srow + j];
 #pragma unroll
 			for (int m = 0; m < GROUP_MAX - 1; m++)
-				if (m < a.nd) a.dst[m][row + j] = v;
+				if (m < a.nd) a.dst[m][drow + j] = v;
 		}
 	}
 }
@@ -189,13 +192,16 @@ cudaError_t launch_carry2_f2(const float2 *src, float2 *dst, long long stride, i
 	k_carry2<float2><<<rows, 128, 0, s>>>(src, dst, stride, src_begin, dst_begin, cnt);
 	return cudaGetLastError();
 }
-cudaError_t launch_c_fanout(const float2 *src, float2 *const *dst, int nd, long long stride, int off, int n, int rows, cudaStream_t s) {
-	if (nd < 1 || nd > GROUP_MAX - 1 || (stride | off | n) & 1) return cudaErrorInvalidValue;
+cudaError_t launch_c_fanout(const float2 *src, long long src_stride, int src_off, float2 *const *dst, int nd, long long dst_stride, int dst_off, int n,
+							int rows, cudaStream_t s) {
+	if (nd < 1 || nd > GROUP_MAX - 1 || (src_stride | dst_stride | src_off | dst_off | n) & 1) return cudaErrorInvalidValue;
 	FanoutArgs a;
 	a.src = reinterpret_cast<const float4 *>(src);
 	for (int m = 0; m < GROUP_MAX - 1; m++) a.dst[m] = m < nd ? reinterpret_cast<float4 *>(dst[m]) : nullptr;
-	a.stride4 = stride / 2;
-	a.off4 = off / 2;
+	a.src_stride4 = src_stride / 2;
+	a.dst_stride4 = dst_stride / 2;
+	a.src_off4 = src_off / 2;
+	a.dst_off4 = dst_off / 2;
 	a.n4 = n / 2;
 	a.rows = rows;
 	a.nd = nd;

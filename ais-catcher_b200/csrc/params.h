@@ -192,10 +192,12 @@ cudaError_t launch_tail_update(void *new_tail, const void *old_tail, const void 
 cudaError_t launch_carry_f2(float2 *buf, long long stride, int src_begin, int dst_begin, int cnt, int rows, cudaStream_t s);
 cudaError_t launch_carry2_f2(const float2 *src, float2 *dst, long long stride, int src_begin, int dst_begin, int cnt, int rows, cudaStream_t s);
 cudaError_t set_taps_bh28_3(const float *taps26);
-// engine groups (aisgpu_attach): float2 elements [off, off + n) of every row of src, n and off even, into the same place of each of
-// the nd (<= GROUP_MAX - 1) buffers dst[]; rows are stride elements apart (even) in all of them
+// engine groups (aisgpu_attach) and the channel dump (aisgpu_dump_open): float2 elements [src_off, src_off + n) of every row of src
+// (rows src_stride apart) into elements [dst_off, dst_off + n) of the same row of each of the nd (<= GROUP_MAX - 1) buffers dst[]
+// (rows dst_stride apart); strides, offsets and n are even
 constexpr int GROUP_MAX = 8; // engines in one group, the leader included
-cudaError_t launch_c_fanout(const float2 *src, float2 *const *dst, int nd, long long stride, int off, int n, int rows, cudaStream_t s);
+cudaError_t launch_c_fanout(const float2 *src, long long src_stride, int src_off, float2 *const *dst, int nd, long long dst_stride, int dst_off, int n,
+							int rows, cudaStream_t s);
 // fe_tiled.cu
 cudaError_t launch_frontend_tiled(const FeParams &p, int fmt, int k, bool pre, dim3 grid, size_t smem, cudaStream_t s);
 // fe_stream_f*.cu: the launcher picks the lanes per stream (st_plan in fe_stream.cuh) unless forced_L > 0

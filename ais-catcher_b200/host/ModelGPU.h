@@ -37,6 +37,8 @@ class ModelGPU : public Model, public StreamIn<RAW> {
 	int granule = 64;                 // samples: every CIC stage needs an even block (DSP.cpp:94,135)
 	size_t blockBytes = 0;            // every submit has this length (fixed by the first Receive, see there)
 	bool failed = false;
+	std::string dumpPrefix;           // -go DUMP <prefix> (Model.cpp:390-396): the 48 kHz channels to <prefix>_A.wav / _B.wav
+	bool dump = false;
 
 	static int formatOf(Format f) {
 		switch (f) {
@@ -65,6 +67,14 @@ class ModelGPU : public Model, public StreamIn<RAW> {
 		if (aisgpu_create(&cfg, &engine) != AISGPU_OK) {
 			fail(std::string("cannot create engine: ") + aisgpu_last_error(nullptr));
 			return false;
+		}
+		// the reference wires the dump behind FilterCIC5 in AB / CD only: in X buildModel returns before it (Model.cpp:106)
+		if (dump && cfg.channel_mode == AISGPU_MODE_AB) {
+			const char *prefixes[1] = { dumpPrefix.c_str() };
+			if (aisgpu_dump_open(engine, prefixes) != AISGPU_OK) {
+				fail(aisgpu_last_error(engine));
+				return false;
+			}
 		}
 		return true;
 	}
@@ -107,7 +117,10 @@ public:
 				: kind == AISGPU_MODEL_STANDARD ? "AIS engine H100 (FM)"
 				: kind == AISGPU_MODEL_DISCRIMINATOR ? "AIS engine H100 (FM discriminator input)" : "AIS engine H100 (FM/PLL)");
 	}
-	~ModelGPU() override { aisgpu_destroy(engine); }
+	~ModelGPU() override {
+		if (engine) aisgpu_dump_close(engine); // completes the WAV headers, as WriteWAV::~WriteWAV does (no-op without a dump)
+		aisgpu_destroy(engine);
+	}
 
 	void buildModel(char CH1, char CH2, int sample_rate, bool timerOn, Device::Device *dev) override {
 		device = dev;
@@ -180,11 +193,14 @@ public:
 		case AIS::KEY_SETTING_DROOP: cfg.droop = Util::Parse::Switch(arg); break;       // ModelFrontend::SetKey, Model.cpp:384-386
 		case AIS::KEY_SETTING_FP_DS: cfg.fp_ds = Util::Parse::Switch(arg); break;       // Model.cpp:362-365 (CU8 @1536K only, as in the reference)
 		case AIS::KEY_SETTING_DSK: cfg.dsk = Util::Parse::Switch(arg); break;           // Model.cpp:377-379
+		case AIS::KEY_SETTING_DUMP: // ModelFrontend::SetKey, Model.cpp:390-396; opened with the engine (ensureEngine)
+			dumpPrefix = arg;
+			dump = true;
+			break;
 		case AIS::KEY_SETTING_SOXR:
 		case AIS::KEY_SETTING_SRC:
 		case AIS::KEY_SETTING_MA:
-		case AIS::KEY_SETTING_DUMP:
-			if (key != AIS::KEY_SETTING_DUMP && !Util::Parse::Switch(arg)) break; // "off" is what the engine does anyway
+			if (!Util::Parse::Switch(arg)) break; // "off" is what the engine does anyway
 			throw std::runtime_error(getName() + ": setting \"" + AIS::KeyMap[key][JSON_DICT_SETTING] + "\" is not available on the GPU engine");
 		default: Model::SetKey(key, arg); break; // STATION_ID, OWN_MMSI, or the reference's "not supported" error
 		}

@@ -68,6 +68,7 @@ extern "C" {
 #define AISGPU_ENOMEM -4   /* device or pinned-host allocation failed */
 #define AISGPU_EOVERFLOW -5 /* returned by aisgpu_poll*(): the frame ring overflowed since the last poll and frames were dropped; the frames
                               that survived were still delivered (out / *n are valid).  Size the ring with aisgpu_config.max_frames. */
+#define AISGPU_EIO -6      /* a channel dump file (aisgpu_dump_open) could not be created or written */
 
 /* tap ids for aisgpu_tap(): intermediates for parity tests */
 #define AISGPU_TAP_C 0     /* 48 kHz channel samples after FilterCIC5 (Model.cpp:345-346 C_a/C_b), float2; AISGPU_MODEL_DISCRIMINATOR:
@@ -301,6 +302,35 @@ int aisgpu_attach(aisgpu_handle *leader, const aisgpu_config *cfg, aisgpu_handle
  * channel_mode, droop, dsk, fp_ds, device -- and neither config may be AISGPU_MODEL_DISCRIMINATOR.  struct_size as for
  * aisgpu_create. */
 int aisgpu_check_attach(const aisgpu_config *leader, const aisgpu_config *member);
+
+/* ---- The 48 kHz channel dump (the reference's -go DUMP <prefix>, Model.cpp:348-353, 390-396) ----
+ *
+ * Writes the two 48 kHz channel streams of stream s (the FilterCIC5 outputs C_a / C_b, what AISGPU_TAP_C reads) to
+ * "<prefixes[s]>_A.wav" (row 2s) and "<prefixes[s]>_B.wav" (row 2s + 1) as Util::WriteWAV does (StreamHelpers.cpp:135-229): a 44-byte
+ * header (IEEE float, 2 channels, 32 bits, 48000 S/s), then every block of samples raw as CF32; the two sizes are patched at close,
+ * as uint32_t.  The letters are A and B in CD mode too.  prefixes[s] == NULL: stream s is not written.  Each file is created at the
+ * first submit that yields 48 kHz samples, and one file descriptor per file stays open until the dump is closed.
+ *
+ * Every submit's rows are gathered on the GPU and copied into one of three pinned slots; the files are written on the caller's
+ * thread, never by a thread of the engine.  The rows of submit t are in the files no later than the return of aisgpu_poll_upto(t),
+ * aisgpu_poll, aisgpu_sync or aisgpu_dump_close; an aisgpu_submit* that needs a slot whose rows have not been written writes them
+ * first.  Frames, taps and counters are the same with and without a dump.
+ *
+ * aisgpu_dump_open is AISGPU_EINVAL, with the handle untouched and the reason in aisgpu_last_error(h), when prefixes is NULL, after
+ * the first submit, when a dump is already open, in AISGPU_MODE_X (the reference writes nothing there, Model.cpp:106), for
+ * AISGPU_MODEL_DISCRIMINATOR (ModelDiscriminator refuses the key, Model.h:107-122) and on a group member (it has no front end: dump
+ * the leader; a leader's dump leaves its members unchanged).  It allocates three device and three pinned slots of
+ * rows x (most 48 kHz samples one submit can yield) CF32 samples.
+ *
+ * A failed create or write stops the dump (the reference's StopRequest()): the reason, in the reference's wording ("WAV out: ..."),
+ * goes to aisgpu_last_error, and every later aisgpu_submit* returns AISGPU_EIO without enqueuing anything until aisgpu_dump_close
+ * has been called.  aisgpu_poll* are not affected and the handle is not poisoned.  aisgpu_feed_files on an engine with an open dump
+ * writes the channels of every block it submits, the zero-padded ones included; AISGPU_EIO is then its first error.
+ *
+ * aisgpu_dump_close writes what is pending, patches the headers and closes the files: 0, or AISGPU_EIO if a create or write failed
+ * (the files are closed with the sizes written so far).  aisgpu_destroy closes an open dump. */
+int aisgpu_dump_open(aisgpu_handle *h, const char *const *prefixes);
+int aisgpu_dump_close(aisgpu_handle *h);
 
 const char *aisgpu_last_error(aisgpu_handle *h); /* h may be NULL: error of the last failed aisgpu_create / aisgpu_attach */
 
