@@ -23,7 +23,7 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_validate", "aisgpu_build_nmea", "aisgpu_chunk_granule", "aisgpu_join", "aisgpu_submit_v", "aisgpu_submit_async",
            "aisgpu_poll_upto", "aisgpu_nccl_unique_id", "aisgpu_comm_init", "aisgpu_allreduce_counts",
            "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
-           "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close"]
+           "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 
@@ -120,6 +120,9 @@ def load():
     if hasattr(lib, "aisgpu_dump_open"):  # absent from libraries built before the channel dump (AISGPU_LIB)
         lib.aisgpu_dump_open.argtypes = [C.c_void_p, C.POINTER(C.c_char_p)]
         lib.aisgpu_dump_close.argtypes = [C.c_void_p]
+    if hasattr(lib, "aisgpu_wav_probe"):  # absent from libraries built before WAV input (AISGPU_LIB)
+        lib.aisgpu_wav_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int32), C.POINTER(C.c_uint32), C.POINTER(C.c_int64)]
+        lib.aisgpu_feed_wav_files.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, MSG_FN, C.c_void_p, C.POINTER(C.c_uint64)]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -156,6 +159,17 @@ def check_device_batch(dev_ptr, stride_samples, sample_rate=1536000, model=MODEL
     rc = lib.aisgpu_check_device_batch(C.byref(cfg), C.c_void_p(dev_ptr), stride_samples)
     if rc:
         raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode()))
+
+
+def wav_probe(path):
+    """aisgpu_wav_probe (no GPU needed): (format, sample_rate, data_offset) of a WAV recording, read as the reference's
+    Device::WAVFile reads it.  Raises with the reference's text if the reference refuses the file."""
+    lib = load()
+    fmt, rate, off = C.c_int32(0), C.c_uint32(0), C.c_int64(0)
+    rc = lib.aisgpu_wav_probe(os.fsencode(path), C.byref(fmt), C.byref(rate), C.byref(off))
+    if rc:
+        raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode()))
+    return fmt.value, rate.value, off.value
 
 
 def make_msg(payload_bytes, nbits, channel="A", start_idx=0, end_idx=0, level=0.0, ppm=0.0, sentences=()):
@@ -329,12 +343,20 @@ class Engine:
 
     def feed_files(self, paths, n):
         """aisgpu_feed_files: one recording per stream, blocks of n samples; returns (messages, blocks submitted)."""
+        return self._feed(self.lib.aisgpu_feed_files, paths, n)
+
+    def feed_wav_files(self, paths, n):
+        """aisgpu_feed_wav_files: one WAV recording per stream, in the engine's format and at its rate, read from its data chunk
+        to its end in blocks of n samples; returns (messages, blocks submitted)."""
+        return self._feed(self.lib.aisgpu_feed_wav_files, paths, n)
+
+    def _feed(self, f, paths, n):
         assert len(paths) == self.n_streams
         arr = (C.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
         out = []
         cb = MSG_FN(lambda msgs, k, user: out.extend(Msg(msgs[i]) for i in range(k)))
         nb = C.c_uint64(0)
-        rc = self.lib.aisgpu_feed_files(self.h, arr, n, cb, None, C.byref(nb))
+        rc = f(self.h, arr, n, cb, None, C.byref(nb))
         if rc == EOVERFLOW:
             self.overflows += 1
         else:

@@ -1614,7 +1614,7 @@ const char *aisgpu_last_error(aisgpu_handle *h) { return h ? h->err.c_str() : g_
 
 // hooks for the host-only units of the library (host_internal.h)
 const aisgpu_config *aisgpu_internal_config(aisgpu_handle *h) { return &h->cfg; }
-void aisgpu_internal_set_error(aisgpu_handle *h, const char *msg) { h->err = msg; }
+void aisgpu_internal_set_error(aisgpu_handle *h, const char *msg) { (h ? h->err : g_create_error) = msg; }
 int aisgpu_internal_grouped(aisgpu_handle *h) { return h->member || !h->members.empty(); }
 
 static int create_impl(aisgpu_handle *h) {

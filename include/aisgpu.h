@@ -285,6 +285,28 @@ int aisgpu_msg_binary(const aisgpu_msg *m, const aisgpu_tag *tag, int crc, uint8
 typedef void (*aisgpu_msg_fn)(const aisgpu_msg *msgs, int n, void *user);
 int aisgpu_feed_files(aisgpu_handle *h, const char *const *paths, int n_samples, aisgpu_msg_fn fn, void *user, uint64_t *n_blocks);
 
+/* == Device::WAVFile::Open (Source/Device/FileWAV.cpp:49-98), host only: reads the header of the WAV file at path as the reference
+ * does, so that a caller can fill aisgpu_config from a recording.  The 12-byte RIFF header must read "RIFF" ... "WAVE"; chunks are
+ * walked until "data", "fmt " may come anywhere before it, and every other chunk is skipped by its size rounded up to an even
+ * number.  The first 16 bytes of "fmt " are read and the rest of it is skipped.  The file must have 2 channels (I/Q), and
+ * tag 3 / 32 bits is AISGPU_FMT_CF32, tag 1 / 8 bits AISGPU_FMT_CU8, tag 1 / 16 bits AISGPU_FMT_CS16; every other format,
+ * WAVE_FORMAT_EXTENSIBLE (0xFFFE) included, is refused.  *sample_rate is dwSamplesPerSec, *data_offset the byte after the data
+ * chunk's header.  The data chunk's size is not read: the samples run from there to the end of the file, so chunks after "data"
+ * (LIST, ...) are read as samples, as WAVFile::isStreaming reads them (FileWAV.cpp:107-120).  A WAV never maps to
+ * AISGPU_FMT_CS8 or AISGPU_FMT_F32_FS4.  AISGPU_EINVAL, with the reference's text in aisgpu_last_error(NULL) ("cannot open WAV
+ * file: ...", "cannot read header from WAV file: ...", "not a supported WAV-file.", "invalid fmt chunk in WAV-file.", "cannot
+ * read fmt chunk from WAV-file.", "no data in WAV-file.", "WAV-file must have 2 channels (I/Q).", "format not supported"), for a
+ * file the reference refuses; the outputs are then untouched. */
+int aisgpu_wav_probe(const char *path, int32_t *format, uint32_t *sample_rate, int64_t *data_offset);
+
+/* == n_streams Device::WAVFile receivers feeding one engine: aisgpu_feed_files with stream s read from the data offset that
+ * aisgpu_wav_probe gives for paths[s] to the end of the file.  The blocks, the zero-padding of each file's tail, the end of the run
+ * with the longest file, fn, *n_blocks and the return values are aisgpu_feed_files's.  Before anything is read or submitted,
+ * every file is probed: one the reference refuses, or one whose format or sample rate differs from the engine's, is AISGPU_EINVAL
+ * with the file and the reason (the reference's text, or the field that differs) in aisgpu_last_error(h).  An engine group is
+ * refused as for aisgpu_feed_files.  AISGPU_MODEL_DISCRIMINATOR reads the stereo recording as I/Q, as ModelDiscriminator does. */
+int aisgpu_feed_wav_files(aisgpu_handle *h, const char *const *paths, int n_samples, aisgpu_msg_fn fn, void *user, uint64_t *n_blocks);
+
 /* ---- Engine groups: several models on one front end (the reference's repeated -m, Receiver.cpp:126-244) ----
  *
  * Makes *out a member of leader's group: an engine with a back end of its own (cfg->model with its own ps_ema, afc_wide, dd_train,
@@ -298,7 +320,7 @@ int aisgpu_feed_files(aisgpu_handle *h, const char *const *paths, int n_samples,
  *     and state: emission order, msg.chunk, sequence ids, AISGPU_EOVERFLOW and the counters are the standalone engine's; counters[2]
  *     and [3] follow the leader's submits;
  *   - only the leader is submitted to (aisgpu_submit, _v, _async, _device); one leader submit runs every member's back end.
- *     aisgpu_submit* on a member, and aisgpu_feed_files on a leader with members, return AISGPU_EINVAL;
+ *     aisgpu_submit* on a member, and aisgpu_feed_files or aisgpu_feed_wav_files on a group's engine, return AISGPU_EINVAL;
  *   - aisgpu_sync(leader) and aisgpu_join(leader) cover the whole group (events on the leader's stream time the group);
  *   - a member has no front end: AISGPU_TAP_ROT, _PRE and _PRE2 are AISGPU_EINVAL, aisgpu_last_frontend_ms() is -1 and
  *     aisgpu_frontend_times() gives n = 0;
