@@ -14,6 +14,7 @@ MODEL_STANDARD, MODEL_BASE, MODEL_DEFAULT, MODEL_CHALLENGER, MODEL_V2 = 0, 1, 2,
 MODEL_DISCRIMINATOR = 3  # FM-discriminator input: I and Q are the audio of two discriminator taps (channels A and B)
 FMT_CF32, FMT_CU8, FMT_CS8, FMT_CS16 = 0, 1, 2, 3
 FMT_F32_FS4 = 4  # one real float32 per sample, made complex by the fs/4 shift 1, j, -1, -j (Airspy / HydraSDR real mode)
+FMT_DC16H = 7  # three uint32 per sample: I and Q are the low 16 bits of words 0 and 1 (Q negated), the rest is not read; 5 and 6 are no formats
 MODE_AB, MODE_X = 0, 3  # aisgpu_config.channel_mode: two channels (also CD) / single channel (-c X)
 TAP_C, TAP_CGF, TAP_FIR, TAP_ROT, TAP_DEC, TAP_FM, TAP_PRE, TAP_PRE2 = 0, 1, 2, 3, 4, 5, 7, 8
 

@@ -73,7 +73,7 @@ constexpr int X_GRANULE = 64; // single-channel mode: a multiple of every format
                               // FM-discriminator input model's granule
 
 int bytes_per_sample(int fmt) { return fe_fmt_bps(fe_fmt_id(fmt)); }
-bool format_known(int fmt) { return fmt >= AISGPU_FMT_CF32 && fmt <= AISGPU_FMT_F32_FS4; }
+bool format_known(int fmt) { return (fmt >= AISGPU_FMT_CF32 && fmt <= AISGPU_FMT_F32_FS4) || fmt == AISGPU_FMT_DC16H; } // 5 and 6 are not formats
 
 // A ring of pre-stage output (Upsample's at the bucket rate, DownsampleKFilter's at 96 kS/s), one row of `stride` samples per stream;
 // positions only grow, position p lives in slot p % cap.
@@ -1322,13 +1322,23 @@ int check_outer(aisgpu_handle *h, int N) {
 //  - the FM-discriminator split at 48 kHz (fe_disc.cu) loads single samples where pairs are not aligned: any sample-aligned base;
 //  - DownsampleKFilter (k_dsk) and the warm-up tail copy (k_tail_update) read single samples;
 //  - F32_FS4: base 16-byte aligned and a stride of whole x, jx, -x, -jx patterns (four samples = 16 bytes), at every rate and in
-//    every mode: each row is then a 16-byte aligned run of whole patterns, which is what every reader above asks for.
+//    every mode: each row is then a 16-byte aligned run of whole patterns, which is what every reader above asks for;
+//  - DC16H: the same rule for another reason -- at 12 bytes per sample four samples are 48 bytes, so a 16-byte aligned base and a
+//    stride that is a multiple of 4 samples put every row on a 16-byte boundary, which the streaming kernels' 16-byte copies need
+//    (the other readers load single 32-bit words).
 int check_placement(aisgpu_handle *h, const void *dev, int64_t stride) {
 	const unsigned long long a = (unsigned long long)(size_t)dev;
 	const int bps = bytes_per_sample(h->cfg.format);
 	if (h->cfg.format == AISGPU_FMT_F32_FS4 && (stride < 0 || stride % 4 || a % 16)) {
 		h->err = "F32_FS4: the base of a device batch must be 16-byte aligned and stride_samples a non-negative multiple of 4";
 		return AISGPU_EINVAL;
+	}
+	if (h->cfg.format == AISGPU_FMT_DC16H) { // the whole rule of the format: "two samples" below would be 24 bytes
+		if (stride < 0 || stride % 4 || a % 16) {
+			h->err = "DC16H: the base of a device batch must be 16-byte aligned and stride_samples a non-negative multiple of 4";
+			return AISGPU_EINVAL;
+		}
+		return 0;
 	}
 	if (stride < 0 || (stride & 1)) {
 		h->err = "stride_samples must be even and non-negative";

@@ -1,4 +1,4 @@
-// fe_common.cuh -- sample-format conversion shared by the front-end kernels (Utilities/Convert.cpp:255-286, and ConvertRAW's
+// fe_common.cuh -- sample-format conversion shared by the front-end kernels (Utilities/Convert.cpp:255-301, and ConvertRAW's
 // F32_FS4 case, Utilities/StreamHelpers.cpp:105-118).
 #pragma once
 #include "exact.cuh"
@@ -16,6 +16,14 @@ __device__ __forceinline__ float fs4_neg(float x) { return __int_as_float(__floa
 __device__ __forceinline__ void fs4_pair(float x0, float x1, bool neg, float2 &a, float2 &b) {
 	a = make_float2(neg ? fs4_neg(x0) : x0, 0.0f);
 	b = make_float2(0.0f, neg ? fs4_neg(x1) : x1);
+}
+
+// DC16H (Convert.cpp:288-301): three 32-bit words per sample.  I is the low half of word 0 and Q the low half of word 1, both
+// sign-extended; the high halves and word 2 are never read.  Q is negated as a 32-bit integer BEFORE the conversion: Q = 0 stays
+// +0.0f (a float negation would make -0.0f, and atan2f tells them apart) and Q = -32768 becomes exactly 1.0f.
+__device__ __forceinline__ float2 dc16h_sample(uint32_t wi, uint32_t wq) {
+	const int i = (int)(short)(wi & 0xFFFFu), q = -(int)(short)(wq & 0xFFFFu);
+	return make_float2(__fmul_rn((float)i, 3.0517578125e-05f), __fmul_rn((float)q, 3.0517578125e-05f));
 }
 
 template <int FMT>
@@ -41,10 +49,15 @@ __device__ __forceinline__ void fe_load_pair(const void *base, long long idx, in
 		a = make_float2(__fmul_rn((float)v.x, 3.0517578125e-05f), __fmul_rn((float)v.y, 3.0517578125e-05f));
 		b = make_float2(__fmul_rn((float)v.z, 3.0517578125e-05f), __fmul_rn((float)v.w, 3.0517578125e-05f));
 	}
-	else { // F32_FS4
-		static_assert(FMT <= 3 || FMT == FE_FMT_FS4, "no conversion for this format id");
+	else if (FMT == FE_FMT_FS4) {
 		const float2 v = __ldg(reinterpret_cast<const float2 *>(reinterpret_cast<const float *>(base) + idx));
 		fs4_pair(v.x, v.y, (pos & 2) != 0, a, b);
+	}
+	else { // DC16H: 24 bytes, read as the four live words (any word-aligned base)
+		static_assert(FMT <= 3 || FMT == FE_FMT_FS4 || FMT == FE_FMT_DC16H, "no conversion for this format id");
+		const uint32_t *w = reinterpret_cast<const uint32_t *>(base) + idx * 3;
+		a = dc16h_sample(__ldg(w), __ldg(w + 1));
+		b = dc16h_sample(__ldg(w + 3), __ldg(w + 4));
 	}
 }
 
@@ -63,10 +76,14 @@ __device__ __forceinline__ float2 fe_load_one(const void *base, long long idx, i
 		const short2 v = __ldg(reinterpret_cast<const short2 *>(base) + idx);
 		return make_float2(__fmul_rn((float)v.x, 3.0517578125e-05f), __fmul_rn((float)v.y, 3.0517578125e-05f));
 	}
-	static_assert(FMT <= 3 || FMT == FE_FMT_FS4, "no conversion for this format id");
-	const float x = __ldg(reinterpret_cast<const float *>(base) + idx);
-	const float y = (pos & 2) ? fs4_neg(x) : x;
-	return (pos & 1) ? make_float2(0.0f, y) : make_float2(y, 0.0f);
+	if (FMT == FE_FMT_FS4) {
+		const float x = __ldg(reinterpret_cast<const float *>(base) + idx);
+		const float y = (pos & 2) ? fs4_neg(x) : x;
+		return (pos & 1) ? make_float2(0.0f, y) : make_float2(y, 0.0f);
+	}
+	static_assert(FMT <= 3 || FMT == FE_FMT_FS4 || FMT == FE_FMT_DC16H, "no conversion for this format id");
+	const uint32_t *w = reinterpret_cast<const uint32_t *>(base) + idx * 3;
+	return dc16h_sample(__ldg(w), __ldg(w + 1));
 }
 
 } // namespace aisgpu

@@ -6,7 +6,8 @@
 //
 // Shape: nothing is recurrent, so one CTA converts one contiguous segment of one stream.  Each thread loads DISC_PAIRS pairs of
 // samples (warp-contiguous) before it stores any, and writes one float2 per pair to each row: every row is written as contiguous
-// 256-byte warp stores.  Pairs are read with one vector load where the batch's rows allow it (CF32 16 bytes, CS16 and F32_FS4 8, CU8/CS8 4).
+// 256-byte warp stores.  Pairs are read with one vector load where the batch's rows allow it (CF32 16 bytes, CS16 and F32_FS4 8, CU8/CS8 4);
+// a DC16H pair is read as its four live words wherever it lies.
 #include "fe_common.cuh"
 #include "params.h"
 
@@ -53,7 +54,7 @@ cudaError_t launch_disc_fmt(const FeParams &p, cudaStream_t s) {
 	const int nseg = (p.N + DISC_SEG - 1) / DISC_SEG;
 	const unsigned ctas = (unsigned)((long long)p.st_B * nseg);
 	// a pair starts at an even sample: one vector load when the batch and its rows are aligned to two samples
-	const bool vec = ((size_t)p.in % (2 * BPS)) == 0 && ((p.in_stride * BPS) % (2 * BPS)) == 0;
+	const bool vec = FMT == FE_FMT_DC16H || (((size_t)p.in % (2 * BPS)) == 0 && ((p.in_stride * BPS) % (2 * BPS)) == 0);
 	if (vec) k_frontend_disc<FMT, true><<<ctas, DISC_THREADS, 0, s>>>(p, nseg);
 	else k_frontend_disc<FMT, false><<<ctas, DISC_THREADS, 0, s>>>(p, nseg);
 	return cudaGetLastError();
@@ -68,6 +69,7 @@ cudaError_t launch_frontend_disc(const FeParams &p, int fmt, cudaStream_t s) {
 	case 2: return launch_disc_fmt<2>(p, s);
 	case 3: return launch_disc_fmt<3>(p, s);
 	case FE_FMT_FS4: return launch_disc_fmt<FE_FMT_FS4>(p, s);
+	case FE_FMT_DC16H: return launch_disc_fmt<FE_FMT_DC16H>(p, s);
 	default: return cudaErrorInvalidValue;
 	}
 }

@@ -168,6 +168,7 @@ cudaError_t launch_dsk(int fmt, const void *in, long long in_stride, const void 
 	case 2: k_dsk<2><<<grid, DSK_THREADS, 0, s>>>(in, in_stride, tail, tail_len, first, n_out, S, s_stride, j0, cap); break;
 	case 3: k_dsk<3><<<grid, DSK_THREADS, 0, s>>>(in, in_stride, tail, tail_len, first, n_out, S, s_stride, j0, cap); break;
 	case FE_FMT_FS4: k_dsk<FE_FMT_FS4><<<grid, DSK_THREADS, 0, s>>>(in, in_stride, tail, tail_len, first, n_out, S, s_stride, j0, cap); break;
+	case FE_FMT_DC16H: k_dsk<FE_FMT_DC16H><<<grid, DSK_THREADS, 0, s>>>(in, in_stride, tail, tail_len, first, n_out, S, s_stride, j0, cap); break;
 	default: return cudaErrorInvalidValue;
 	}
 	return cudaGetLastError();

@@ -86,9 +86,14 @@ __device__ __forceinline__ c64 u16pair_to_c64(uint32_t z) {
 template <int FMT, int G>
 struct StFmt {
 	static constexpr int BPS = fe_fmt_bps(FMT);   // FMT 4: CU8 through the integer CIC stages (-go FP_DS on)
-	static constexpr int CHUNK = G * BPS;         // bytes of one lane's chunk (G = 16: 128 / 32 / 32 / 64)
-	static constexpr int PIECES = CHUNK / 16;     // 16-byte pieces per lane chunk = cp.async instructions per warp chunk
+	static constexpr int CHUNK = G * BPS;         // bytes of one lane's chunk (G = 16: 128 / 32 / 32 / 64; DC16H 192)
+	// The staging below deals the 16-byte pieces of 32 / PIECES owners' chunks to the 32 lanes of one cp.async instruction, so PIECES
+	// has to divide 32.  DC16H's 12 bytes per sample give a chunk a factor 3: it is staged as PARTS = 3 consecutive thirds, each a
+	// chunk of PIECES pieces with the same lane-to-owner mapping (16 samples: three 64-byte thirds of 4 pieces).
+	static constexpr int PARTS = BPS % 3 == 0 ? 3 : 1;
+	static constexpr int PIECES = CHUNK / PARTS / 16; // 16-byte pieces per part; PARTS * PIECES cp.async instructions per warp chunk
 	static constexpr int SLOT = CHUNK + 16;       // lane stride in the ring (odd multiple of 16 bytes: conflict-free 16-byte reads)
+	static_assert(PIECES >= 1 && 32 % PIECES == 0 && (SLOT / 16) % 2 == 1, "staging shape");
 };
 // sample pair j (samples 2j, 2j+1) of a staged chunk.  F32_FS4: a chunk starts at a multiple of 4 samples of the submit (the
 // kernels assert what that rests on), so the pair's place in the x, jx, -x, -jx pattern is j & 1.
@@ -114,11 +119,30 @@ __device__ __forceinline__ void st_read_pair(const unsigned char *slot, int j, c
 		xe = pack2(__fmul_rn((float)v.x, 3.0517578125e-05f), __fmul_rn((float)v.y, 3.0517578125e-05f));
 		xo = pack2(__fmul_rn((float)v.z, 3.0517578125e-05f), __fmul_rn((float)v.w, 3.0517578125e-05f));
 	}
-	else {
-		static_assert(FMT <= 3 || FMT == FE_FMT_FS4, "no conversion for this format id");
+	else if (FMT == FE_FMT_FS4) {
 		const float2 v = *reinterpret_cast<const float2 *>(slot + j * 8);
 		float2 a, b;
 		fs4_pair(v.x, v.y, (j & 1) != 0, a, b);
+		xe = pack2(a.x, a.y);
+		xo = pack2(b.x, b.y);
+	}
+	else { // DC16H: the pair's six words lie in the 48-byte quad (j / 2) of the slot, which is 16-byte aligned
+		static_assert(FMT <= 3 || FMT == FE_FMT_FS4 || FMT == FE_FMT_DC16H, "no conversion for this format id");
+		// words 0 1 (2) 3 | 4 (5) 6 7 | (8) 9 10 (11) of a quad are the I and Q of its samples 0 .. 3; the callers' pair loops are
+		// unrolled, so the loads of the middle 16 bytes are shared by the quad's two pairs
+		const uint4 *q = reinterpret_cast<const uint4 *>(slot + (j >> 1) * 48);
+		const uint4 m = q[1];
+		float2 a, b;
+		if ((j & 1) == 0) {
+			const uint4 v = q[0];
+			a = dc16h_sample(v.x, v.y);
+			b = dc16h_sample(v.w, m.x);
+		}
+		else {
+			const uint4 v = q[2];
+			a = dc16h_sample(m.z, m.w);
+			b = dc16h_sample(v.y, v.z);
+		}
 		xe = pack2(a.x, a.y);
 		xo = pack2(b.x, b.y);
 	}
@@ -160,7 +184,8 @@ __global__ void __launch_bounds__(ST_WARPS * 32) k_frontend_st(const FeParams p)
 	const long long a = ((long long)sub * p.st_q + max(0, sub - n_short)) * SS;
 	const int n_super = p.P / SS + p.st_q + (p.st_r ? 1 : 0);
 	const int warp_chunks = n_super * NCH; // warm-up included
-	// staging: in instruction `it` lane j fetches 16-byte piece (j % PIECES) of the chunk of owner it*(32/PIECES) + j / PIECES;
+	// staging: in instruction `it` lane j fetches 16-byte piece (j % PIECES) of the chunk (DC16H: of each third of the chunk) of owner
+	// it*(32/PIECES) + j / PIECES;
 	// only the first sub-segment of a stream starts in the previous submit: its warm-up chunks come from the tail buffer
 	constexpr int OWN_PER_IT = 32 / F::PIECES;
 	const int o0 = lane / F::PIECES, q0 = lane % F::PIECES;
@@ -185,14 +210,20 @@ __global__ void __launch_bounds__(ST_WARPS * 32) k_frontend_st(const FeParams p)
 #pragma unroll 1
 				for (int it = 0; it < F::PIECES; it++) {
 					const unsigned long long w = __shfl_sync(0xffffffffu, my_warm, it * OWN_PER_IT + o0);
-					cp_async16(dst + it * OWN_PER_IT * F::SLOT, reinterpret_cast<const unsigned char *>(w) + coff);
+#pragma unroll
+					for (int t = 0; t < F::PARTS; t++)
+						cp_async16(dst + it * OWN_PER_IT * F::SLOT + t * F::PIECES * 16, reinterpret_cast<const unsigned char *>(w) + coff + t * F::PIECES * 16);
 				}
 			}
 			else {
 				unsigned long long base = (unsigned long long)(in0 + coff);
 				asm volatile("" : "+l"(base)); // one register pair: otherwise ptxas keeps p.in uniform and adds it to every address again
 #pragma unroll
-				for (int it = 0; it < F::PIECES; it++) cp_async16(dst + it * OWN_PER_IT * F::SLOT, reinterpret_cast<const unsigned char *>(base + ((unsigned long long)own_off[it] << 4)));
+				for (int t = 0; t < F::PARTS; t++) {
+#pragma unroll
+					for (int it = 0; it < F::PIECES; it++)
+						cp_async16(dst + it * OWN_PER_IT * F::SLOT + t * F::PIECES * 16, reinterpret_cast<const unsigned char *>(base + ((unsigned long long)own_off[it] << 4)) + t * F::PIECES * 16);
+				}
 			}
 		}
 		cp_async_commit();
@@ -423,11 +454,13 @@ cudaError_t launch_frontend_stream_shape(const FeParams &p, int k, bool pre, int
 	default: return cudaErrorNotSupported;
 	}
 }
-// The shapes that exist, each compiled by its own translation unit only (fe_stream_f0e.cu .. fe_stream_f3.cu, fe_stream_fs4.cu)
+// The shapes that exist, each compiled by its own translation unit only (fe_stream_f0e.cu .. fe_stream_f3.cu, fe_stream_fs4.cu,
+// fe_stream_dc16h.cu)
 extern template cudaError_t launch_frontend_stream_shape<0, 32, 3, 4>(const FeParams &, int, bool, int, cudaStream_t);
 extern template cudaError_t launch_frontend_stream_shape<1, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
 extern template cudaError_t launch_frontend_stream_shape<2, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
 extern template cudaError_t launch_frontend_stream_shape<3, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
 extern template cudaError_t launch_frontend_stream_shape<FE_FMT_FS4, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
+extern template cudaError_t launch_frontend_stream_shape<FE_FMT_DC16H, 16, 8, 1>(const FeParams &, int, bool, int, cudaStream_t);
 
 } // namespace aisgpu

@@ -16,6 +16,8 @@ cudaError_t launch_frontend_stream(const FeParams &p, int fmt, int k, bool pre, 
 	case 2: return launch_frontend_stream_shape<2, 16, 8, 1>(p, k, pre, forced_L, s);
 	case 3: return launch_frontend_stream_shape<3, 16, 8, 1>(p, k, pre, forced_L, s);
 	case FE_FMT_FS4: return launch_frontend_stream_shape<FE_FMT_FS4, 16, 8, 1>(p, k, pre, forced_L, s); // CS16's bytes per sample: CS16's shape (the CF32 shape was not measured for it)
+	// 12 bytes per sample: CS16's chunk length, ring depth and one-warp CTAs (the one shape measured); its ring is 52 KB per CTA
+	case FE_FMT_DC16H: return launch_frontend_stream_shape<FE_FMT_DC16H, 16, 8, 1>(p, k, pre, forced_L, s);
 	default: return cudaErrorInvalidValue;
 	}
 }

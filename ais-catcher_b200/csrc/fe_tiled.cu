@@ -182,7 +182,7 @@ __global__ void __launch_bounds__(NW * 32) k_frontend(const FeParams p) {
 		const int b = t & 1;
 		if (tid == 0 && t + 1 < n_tiles) issue(t + 1); // ring slot b^1 was released by the barriers of tile t-1
 		const int off_in = (b ? p.off_in[1] : p.off_in[0]) + FE_HIST;
-		if (FMT != 0) { // integer formats and F32_FS4: convert while loading (registers), no bulk copy
+		if (FMT != 0) { // integer formats, F32_FS4 and DC16H: convert while loading (registers), no bulk copy
 			// F32_FS4: pos, the tile's first sample relative to the submit, is a multiple of 4 -- seg_len is whole tiles, a tile a whole
 			// number of super-steps (or the whole block), P a whole number of super-steps -- but the pattern position is taken from
 			// pos + i itself, so nothing here depends on it
@@ -309,6 +309,7 @@ cudaError_t launch_frontend_tiled(const FeParams &p, int fmt, int k, bool pre, d
 	case 2: return launch_tiled_fmt<2>(p, k, pre, grid, smem, s);
 	case 3: return launch_tiled_fmt<3>(p, k, pre, grid, smem, s);
 	case FE_FMT_FS4: return launch_tiled_fmt<FE_FMT_FS4>(p, k, pre, grid, smem, s);
+	case FE_FMT_DC16H: return launch_tiled_fmt<FE_FMT_DC16H>(p, k, pre, grid, smem, s);
 	default: return cudaErrorInvalidValue;
 	}
 }

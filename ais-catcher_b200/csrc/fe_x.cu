@@ -5,7 +5,8 @@
 //
 // Shape: the per-thread streaming pipeline of fe_stream.cuh without Rotate.  Every lane owns a sub-segment of one stream and
 // walks it chunk by chunk with the filter state in registers, after P samples of warm-up from zero state (every stage is a pure
-// function of its last few inputs).  A chunk is 128 bytes of input per lane (16 CF32, 32 CS16 or F32_FS4, 64 CU8/CS8 samples); the warp
+// function of its last few inputs).  A chunk is 128 bytes of input per lane (16 CF32, 32 CS16 or F32_FS4, 64 CU8/CS8 samples; DC16H:
+// 16 samples = 192 bytes, staged as three 64-byte thirds like the streaming front end's, StFmt in fe_stream.cuh); the warp
 // stages the chunks of its 32 lanes through a shared-memory ring with coalesced 16-byte cp.async copies, NB - 1 chunks ahead.
 // Each input byte is read once, plus P samples per sub-segment.  The lanes per stream come from the same planner as the
 // streaming front end (st_plan): as few as give one balanced wave over the SMs.
@@ -20,9 +21,9 @@ constexpr int X_NB = 6; // chunks in a warp's staging ring (5 in flight while on
 template <int FMT>
 struct XFmt {
 	static constexpr int BPS = fe_fmt_bps(FMT);
-	static constexpr int G = 128 / BPS; // samples per lane chunk (a multiple of 4: an F32_FS4 chunk starts at pattern position 0, as a
-	                                    // lane's a and P are whole chunks)
-	typedef StFmt<FMT, G> F;            // CHUNK = 128 bytes, PIECES = 8, SLOT = 144
+	static constexpr int G = BPS == 12 ? 16 : 128 / BPS; // samples per lane chunk (a multiple of 4: an F32_FS4 chunk starts at pattern
+	                                                     // position 0, as a lane's a and P are whole chunks)
+	typedef StFmt<FMT, G> F;            // CHUNK = 128 bytes, PIECES = 8, SLOT = 144 (DC16H: 192 bytes, 3 parts of 4 pieces, SLOT = 208)
 };
 
 template <int FMT, int K>
@@ -51,7 +52,7 @@ __global__ void __launch_bounds__(32) k_frontend_x(const FeParams p) {
 												: (unsigned long long)in_row;
 	const unsigned long long my_main = (unsigned long long)in_row;
 	// instruction `it` of a chunk: lane j copies 16-byte piece (j % 8) of the chunk of owner it * 4 + j / 8 -- four owners' 128-byte
-	// chunks per warp instruction
+	// chunks per warp instruction (DC16H: piece j % 4 of each third of the chunk of owner it * 8 + j / 4)
 	constexpr int OWN_PER_IT = 32 / F::PIECES;
 	const int o0 = lane / F::PIECES, q0 = lane % F::PIECES;
 	unsigned char(*ring)[32 * F::SLOT] = reinterpret_cast<unsigned char(*)[32 * F::SLOT]>(x_ring);
@@ -62,7 +63,9 @@ __global__ void __launch_bounds__(32) k_frontend_x(const FeParams p) {
 #pragma unroll
 			for (int it = 0; it < F::PIECES; it++) {
 				const unsigned long long w = __shfl_sync(0xffffffffu, base, it * OWN_PER_IT + o0);
-				cp_async16(dst + it * OWN_PER_IT * F::SLOT, reinterpret_cast<const unsigned char *>(w) + (long long)c * F::CHUNK + q0 * 16);
+#pragma unroll
+				for (int t = 0; t < F::PARTS; t++)
+					cp_async16(dst + it * OWN_PER_IT * F::SLOT + t * F::PIECES * 16, reinterpret_cast<const unsigned char *>(w) + (long long)c * F::CHUNK + q0 * 16 + t * F::PIECES * 16);
 			}
 		}
 		cp_async_commit();
@@ -159,7 +162,7 @@ cudaError_t launch_x_fmt(const FeParams &p, int k, int forced_L, cudaStream_t s)
 
 } // namespace
 
-int frontend_x_granule(int fmt) { return 128 / fe_fmt_bps(fmt); }
+int frontend_x_granule(int fmt) { return fmt == FE_FMT_DC16H ? XFmt<FE_FMT_DC16H>::G : 128 / fe_fmt_bps(fmt); }
 
 cudaError_t launch_frontend_x(const FeParams &p, int fmt, int k, int forced_L, cudaStream_t s) {
 	switch (fmt) {
@@ -168,6 +171,7 @@ cudaError_t launch_frontend_x(const FeParams &p, int fmt, int k, int forced_L, c
 	case 2: return launch_x_fmt<2>(p, k, forced_L, s);
 	case 3: return launch_x_fmt<3>(p, k, forced_L, s);
 	case FE_FMT_FS4: return launch_x_fmt<FE_FMT_FS4>(p, k, forced_L, s);
+	case FE_FMT_DC16H: return launch_x_fmt<FE_FMT_DC16H>(p, k, forced_L, s);
 	default: return cudaErrorInvalidValue;
 	}
 }

@@ -62,7 +62,7 @@ int feed(aisgpu_handle *h, const char *who, const char *const *paths, const int6
 	if (int rc = check_args(h, who, paths, n_samples)) return rc;
 	const aisgpu_config *cfg = aisgpu_internal_config(h);
 	const int B = cfg->n_streams;
-	const size_t bps = cfg->format == AISGPU_FMT_CF32 ? 8 : ((cfg->format == AISGPU_FMT_CS16 || cfg->format == AISGPU_FMT_F32_FS4) ? 4 : 2);
+	const size_t bps = cfg->format == AISGPU_FMT_CF32 ? 8 : (cfg->format == AISGPU_FMT_DC16H ? 12 : ((cfg->format == AISGPU_FMT_CS16 || cfg->format == AISGPU_FMT_F32_FS4) ? 4 : 2));
 	const size_t block_bytes = (size_t)n_samples * bps;
 	std::vector<Source> src((size_t)B);
 	auto close_all = [&]() {
@@ -196,6 +196,7 @@ const char *format_name(int32_t f) {
 	case AISGPU_FMT_CS8: return "CS8";
 	case AISGPU_FMT_CS16: return "CS16";
 	case AISGPU_FMT_F32_FS4: return "F32_FS4";
+	case AISGPU_FMT_DC16H: return "DC16H";
 	default: return "?";
 	}
 }

@@ -1,7 +1,7 @@
 // params.h -- parameter blocks, per-row state records and launch entry points of the kernels (host and device view).
 //
 // Layout in HBM (one engine == one batch of B independent IQ streams, "row" = stream*2 + channel; single-channel mode: row = stream):
-//   in     [B][N]              input samples of one submit (CF32 float2, CU8/CS8/CS16, or F32_FS4 floats)
+//   in     [B][N]              input samples of one submit (CF32 float2, CU8/CS8/CS16, F32_FS4 floats, or DC16H word triples)
 //   tail   [B][P]              last P input samples of the previous submit (front-end warm-up history)
 //   rot    [P96 + N>>k]        Rotate phasor table of the submit (shared by all streams), with P96 history
 //   Cbuf   [2B][HC + n48max]   48 kHz channel samples; new samples land at offset HC, unconsumed/history before (FM-discriminator
@@ -20,11 +20,13 @@ constexpr int FE_SLACK = 12; // over-read room behind each array for partial run
 constexpr int FE_MAXK = 7;
 
 // The kernels' FMT template parameter.  0 .. 3 are the public AISGPU_FMT_* values; 4 is CU8 through the integer CIC stages
-// (-go FP_DS on, fe_stream.cuh), so F32_FS4 (public value 4) has an id of its own.  fe_fmt_id is the one place the public value
-// is translated: every launch entry point below takes its result.
-constexpr int FE_FMT_FPDS = 4, FE_FMT_FS4 = 5;
-inline int fe_fmt_id(int public_format) { return public_format == 4 ? FE_FMT_FS4 : public_format; }
-__host__ __device__ constexpr int fe_fmt_bps(int fmt) { return fmt == 0 ? 8 : ((fmt == 3 || fmt == FE_FMT_FS4) ? 4 : 2); } // bytes per sample
+// (-go FP_DS on, fe_stream.cuh), so F32_FS4 (public value 4) and DC16H (public value 7) have ids of their own.  fe_fmt_id is the
+// one place the public value is translated: every launch entry point below takes its result.
+constexpr int FE_FMT_FPDS = 4, FE_FMT_FS4 = 5, FE_FMT_DC16H = 6;
+inline int fe_fmt_id(int public_format) { return public_format == 4 ? FE_FMT_FS4 : (public_format == 7 ? FE_FMT_DC16H : public_format); }
+__host__ __device__ constexpr int fe_fmt_bps(int fmt) { // bytes per sample
+	return fmt == 0 ? 8 : (fmt == FE_FMT_DC16H ? 12 : ((fmt == 3 || fmt == FE_FMT_FS4) ? 4 : 2));
+}
 
 struct FeParams {
 	const void *in;       // [B][in_stride] samples

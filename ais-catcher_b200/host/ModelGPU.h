@@ -47,10 +47,13 @@ class ModelGPU : public Model, public StreamIn<RAW> {
 		case Format::CS8: return AISGPU_FMT_CS8;
 		case Format::CS16: return AISGPU_FMT_CS16;
 		case Format::F32_FS4: return AISGPU_FMT_F32_FS4;
+		case Format::DC16H: return AISGPU_FMT_DC16H;
 		default: return -1;
 		}
 	}
-	static int bytesPerSample(int fmt) { return fmt == AISGPU_FMT_CF32 ? 8 : ((fmt == AISGPU_FMT_CS16 || fmt == AISGPU_FMT_F32_FS4) ? 4 : 2); }
+	static int bytesPerSample(int fmt) {
+		return fmt == AISGPU_FMT_CF32 ? 8 : (fmt == AISGPU_FMT_DC16H ? 12 : ((fmt == AISGPU_FMT_CS16 || fmt == AISGPU_FMT_F32_FS4) ? 4 : 2));
+	}
 
 	void fail(const std::string &what) {
 		if (!failed) Error() << "ModelGPU: " << what;
@@ -164,6 +167,9 @@ public:
 		// starts the 1, j, -1, -j pattern again with the next buffer.  With them dropped here every buffer adds a whole number of
 		// patterns, and the blocks below are multiples of the granule (a multiple of 4): the re-blocking keeps every sample's place.
 		if (cfg.format == AISGPU_FMT_F32_FS4) n = n / 16 * 16;
+		// DC16H: ConvertRAW takes size / 12 samples of a buffer (StreamHelpers.cpp:120-126); the bytes short of a sample are dropped,
+		// not carried into the next buffer
+		if (cfg.format == AISGPU_FMT_DC16H) n = n / 12 * 12;
 		if (!blockBytes) {
 			size_t samples = n / bps / granule * granule;
 			if (samples < (size_t)granule) samples = (size_t)granule;

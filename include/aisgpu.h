@@ -55,7 +55,7 @@ extern "C" {
  * 4-byte elements), AISGPU_TAP_FIR the Filter 37 output, AISGPU_TAP_PRE the Upsample output (float2, both channels), tap 4 the
  * per-phase decoder input; AISGPU_TAP_ROT, AISGPU_TAP_CGF and AISGPU_TAP_PRE2 are AISGPU_EINVAL. */
 
-/* input sample formats: the formats of enum class Format (Source/Library/Common.h:89-104) that ConvertRAW takes, but DC16H */
+/* input sample formats: the formats of enum class Format (Source/Library/Common.h:89-104) that ConvertRAW takes */
 #define AISGPU_FMT_CF32 0
 #define AISGPU_FMT_CU8 1
 #define AISGPU_FMT_CS8 2
@@ -67,8 +67,18 @@ extern "C" {
  * real sample gives one complex sample, and the rate -> chain table, the granules and every mode and model apply unchanged
  * (AISGPU_MODEL_DISCRIMINATOR reads the real / imaginary parts of the expanded samples like ModelDiscriminator's own ConvertRAW).
  * The pattern restarts with every submit; every granule is a multiple of 4, so a sample's place in it is its index in the submit
- * modulo 4.  A submit of n_samples is n_samples floats per stream.  Value 5 is left free (Format::DC16H is not supported). */
+ * modulo 4.  A submit of n_samples is n_samples floats per stream. */
 #define AISGPU_FMT_F32_FS4 4
+/* Format::DC16H (typedef uint32_t DC16H[3], Source/Library/Common.h:87; Convert::toFloat, Source/Utilities/Convert.cpp:288-301):
+ * THREE 32-bit words per sample, 12 bytes.  I is the sign-extended low 16 bits of word 0, Q the sign-extended low 16 bits of word 1;
+ * the high halves of both and the whole of word 2 are never read.  re = I / 32768, im = (-Q) / 32768 with Q negated as a 32-bit
+ * integer before the division: Q = 0 gives +0.0f (never -0.0f) and Q = -32768 gives exactly 1.0f.  It is what -gr FORMAT DC16H reads
+ * from a recording (Utilities/Parse.cpp:188-189); ConvertRAW takes size / 12 samples of a buffer and drops the bytes short of one
+ * (StreamHelpers.cpp:120-126).  sample_rate is the rate of the complex samples; the rate -> chain table, the granules and every
+ * mode, model and switch apply unchanged, FP_DS as for CS16 and CF32 (the integer CIC stages take CU8 only, Model.cpp:231-237).
+ * A submit of n_samples is 3 * n_samples words per stream.  aisgpu_wav_probe never returns it (no WAV layout maps to it).
+ * Its value is 7: 5 and 6 are not formats and stay AISGPU_EINVAL ("bad format"), the answer callers have always had for them. */
+#define AISGPU_FMT_DC16H 7
 
 #define AISGPU_OK 0
 #define AISGPU_EINVAL -1   /* bad argument / unsupported configuration (reference: std::runtime_error at buildModel, Model.cpp:109-110) */
@@ -185,7 +195,9 @@ int aisgpu_submit_async(aisgpu_handle *h, const void *host_samples, int n_sample
  *   - AISGPU_MODE_X and FP_DS: dev_samples and every row are 16-byte aligned (stride_samples * bytes per sample % 16 == 0);
  *   - AISGPU_MODEL_DISCRIMINATOR at exactly 48000 S/s: dev_samples only needs to be aligned to one sample;
  *   - AISGPU_FMT_F32_FS4, in every mode and model: dev_samples is 16-byte aligned and stride_samples is a multiple of 4, so every row
- *     starts a new 1, j, -1, -j pattern on a 16-byte boundary. */
+ *     starts a new 1, j, -1, -j pattern on a 16-byte boundary;
+ *   - AISGPU_FMT_DC16H, in every mode and model: dev_samples is 16-byte aligned and stride_samples is a multiple of 4 (four samples
+ *     are 48 bytes), so every row starts on a 16-byte boundary. */
 int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stride_samples, int n_samples);
 
 /* The placement rule of aisgpu_submit_device for an engine created with *cfg, without touching the GPU (dev_samples is only
@@ -277,7 +289,8 @@ int aisgpu_msg_json(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int c
 int aisgpu_msg_binary(const aisgpu_msg *m, const aisgpu_tag *tag, int crc, uint8_t *out, int cap);
 
 /* == n_streams Device::RAWFile receivers (Source/Device/FileRAW.cpp:36-165) feeding one engine: paths[s] is the recording of
- * stream s in the engine's sample format (F32_FS4: 4-byte real samples; the padding is +0 floats); the files are read in blocks of n_samples (a multiple of aisgpu_chunk_granule),
+ * stream s in the engine's sample format (F32_FS4: 4-byte real samples; the padding is +0 floats.  DC16H: 12-byte samples;
+ * the padding is zero words, samples (+0, +0)); the files are read in blocks of n_samples (a multiple of aisgpu_chunk_granule),
  * the tail of each file is zero-padded to a whole block (FileRAW.cpp:91-94) and the run ends with the longest file.  Reading
  * block c+1 (threads), the copy and kernels of block c and the delivery of the frames of block c-1 to fn overlap (two pinned
  * buffers, aisgpu_submit_async / aisgpu_poll_upto).  fn may be NULL (count only: aisgpu_counters).  *n_blocks receives the
