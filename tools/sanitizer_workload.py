@@ -131,4 +131,22 @@ for c, (stride, off) in enumerate(((N + 4, 0), (N + 64, 16), (3 * N, 16), (N, 0)
     del dev
 print("padded-stride F32_FS4 device batch messages", len(eng.poll()))
 eng.close()
+import afc_signals  # frequency correction: carriers across the whole AFC range, and the V2 engine's slot-locked split
+nw = afc_signals.SWEEP_N48 * 32
+xw = np.stack(afc_signals.rows(fs, nw, afc_signals.COARSE[::4] + afc_signals.FINE_WIDE[::6]) + [afc_signals.edge_tones(fs, nw, 0, 0)])
+for model in (aisgpu.MODEL_DEFAULT, aisgpu.MODEL_V2):
+    eng = aisgpu.Engine(model=model, sample_rate=fs, n_streams=len(xw), max_chunk=N, taps=True)
+    for c in range(nw // N):
+        eng.submit(np.ascontiguousarray(xw[:, c * N:(c + 1) * N]), N)
+    print("wide-offset sweep model", model, "messages", len(eng.poll()))
+    eng.close()
+ns = afc_signals.SLOT_N48 * 32
+xl = np.stack([afc_signals.slotted(fs, ns, ph, k) for k, ph in enumerate(afc_signals.SLOT_PHASES[afc_signals.AB])])
+eng = aisgpu.Engine(model=aisgpu.MODEL_V2, sample_rate=fs, n_streams=len(xl), max_chunk=N + 8192)
+o = 0
+for n in [N, N + 8192, 64 * 5] * (ns // (2 * N + 8192 + 320)):  # locked blocks end a submit at any point of the slot cycle
+    eng.submit(np.ascontiguousarray(xl[:, o:o + n]), n)
+    o += n
+print("slot-locked V2 messages", len(eng.poll()))
+eng.close()
 print("sanitizer workload done")
