@@ -24,7 +24,8 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_validate", "aisgpu_build_nmea", "aisgpu_chunk_granule", "aisgpu_join", "aisgpu_submit_v", "aisgpu_submit_async",
            "aisgpu_poll_upto", "aisgpu_nccl_unique_id", "aisgpu_comm_init", "aisgpu_allreduce_counts",
            "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
-           "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files"]
+           "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files",
+           "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 
@@ -55,7 +56,7 @@ MSG_FN = C.CFUNCTYPE(None, C.POINTER(MsgStruct), C.c_int, C.c_void_p)
 
 
 class Msg:
-    __slots__ = ("stream", "channel", "nbits", "start_idx", "end_idx", "level", "ppm", "chunk", "payload", "nmea")
+    __slots__ = ("stream", "channel", "nbits", "start_idx", "end_idx", "level", "ppm", "chunk", "payload", "nmea", "data")
 
     def __init__(self, m):
         self.stream = m.stream
@@ -68,6 +69,7 @@ class Msg:
         self.chunk = m.chunk
         self.payload = bytes(m.data[:(m.nbits + 7) // 8])
         self.nmea = [m.nmea[i].raw[:m.nmea_len[i]].decode("latin-1") for i in range(min(m.n_sentences, 4))]
+        self.data = bytes(m.data)  # all of aisgpu_msg::data: the full JSON reads bits past nbits as the reference does
 
     def key(self):
         return (self.channel, self.nbits, self.payload, tuple(self.nmea))
@@ -124,6 +126,10 @@ def load():
     if hasattr(lib, "aisgpu_wav_probe"):  # absent from libraries built before WAV input (AISGPU_LIB)
         lib.aisgpu_wav_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int32), C.POINTER(C.c_uint32), C.POINTER(C.c_int64)]
         lib.aisgpu_feed_wav_files.argtypes = [C.c_void_p, C.POINTER(C.c_char_p), C.c_int, MSG_FN, C.c_void_p, C.POINTER(C.c_uint64)]
+    if hasattr(lib, "aisgpu_msg_json_full"):  # absent from libraries built before the full JSON (AISGPU_LIB)
+        lib.aisgpu_msg_json_full.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
+        lib.aisgpu_json_enable.argtypes = [C.c_void_p, C.POINTER(TagStruct), C.c_int]
+        lib.aisgpu_poll_json.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int)]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -202,6 +208,25 @@ def msg_json(m, tag, cap=4096):
     if n < 0:
         raise AisGpuError("aisgpu_msg_json rc=%d" % n)
     return buf.raw[:n]
+
+
+def msg_json_full(m, tag, cap=65536):
+    """Host-only: aisgpu_msg_json_full (the reference's JSONAIS line, JSON::Serializer(JSON_DICT_FULL)) -> bytes.
+    m: an aisgpu_msg (make_msg) or a polled Msg."""
+    if isinstance(m, Msg):
+        m = msg_struct(m)
+    buf = C.create_string_buffer(cap)
+    n = load().aisgpu_msg_json_full(C.byref(m), C.byref(tag), buf, cap)
+    if n < 0:
+        raise AisGpuError("aisgpu_msg_json_full rc=%d" % n)
+    return buf.raw[:n]
+
+
+def msg_struct(msg):
+    """The aisgpu_msg of a polled Msg (every byte of data, the sentences, channel, level, ppm, indices)."""
+    m = make_msg(msg.data, msg.nbits, msg.channel, msg.start_idx, msg.end_idx, msg.level, msg.ppm, msg.nmea)
+    m.stream, m.chunk = msg.stream, msg.chunk
+    return m
 
 
 def msg_binary(m, tag, crc, cap=1024):
@@ -404,6 +429,25 @@ class Engine:
 
     def sync(self):
         self._chk(self.lib.aisgpu_sync(self.h))
+
+    def json_enable(self, tag=None, max_bytes_per_submit=1 << 24):
+        """aisgpu_json_enable: from the first submit on, every polled frame is also decoded into the full AIS JSON on the GPU
+        with tag (make_tag(); default: make_tag()), at most max_bytes_per_submit bytes of lines per submit."""
+        self._json_tag = tag if tag is not None else make_tag()  # the tag's strings must outlive the call only; kept anyway
+        self._chk(self.lib.aisgpu_json_enable(self.h, C.byref(self._json_tag), int(max_bytes_per_submit)))
+
+    def poll_json(self, ticket=None, cap=1 << 20):
+        """aisgpu_poll_json: the lines (str, UTF-8) of the frames of the submits up to ticket (None: all), in frame order."""
+        t = -1 if ticket is None else int(ticket)
+        buf = C.create_string_buffer(cap)
+        nb, nl = C.c_size_t(0), C.c_int(0)
+        out = []
+        while True:
+            self._chk(self.lib.aisgpu_poll_json(self.h, t, buf, cap, C.byref(nb), C.byref(nl)))
+            if nl.value == 0:
+                break
+            out.extend(buf.raw[:nb.value].decode("utf-8", "surrogateescape").split("\n")[:-1])
+        return out
 
     def poll(self, batch=256):
         out = []

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/aisgpu.h"
+#include "be_json.h"
 #include "dump.h"
 #include "params.h"
 
@@ -288,6 +289,28 @@ struct aisgpu_handle {
 	std::deque<DumpPending> dump_pending; // slots copied or being copied, not yet written, in submit order
 	int dump_slot = -1;                   // the submit being enqueued: its slot (-1: no export), row length and columns exported so far
 	long long dump_n = 0, dump_off = 0;
+	// The full AIS JSON (aisgpu_json_enable).  Every drain of the frame ring uploads the frames it publishes to d_jmsg, kJsonBatch
+	// at a time, and decodes them on json_stream (be_json.cu: a line per frame into its slot, the placement within json_cap bytes
+	// per submit, the packed text); the text comes back through pin_jtext and is appended to json_buf, which aisgpu_poll_json hands
+	// out from json_pos on.  Frames and lines are queued side by side and each is read by its own poll; neither queue keeps more
+	// than ring_cap unread entries (json_lines counts the unread lines): the oldest are dropped and the next poll of that kind
+	// returns AISGPU_EOVERFLOW.  Nothing of this exists while JSON has not been enabled.
+	bool json_on = false;
+	int json_mode = 0, json_station = 0, json_slot = 0;
+	long long json_cap = 0;
+	std::string json_prefix;
+	cudaStream_t json_stream = nullptr;
+	char *d_jprefix = nullptr, *d_jslots = nullptr, *d_jtext = nullptr;
+	aisgpu_msg *d_jmsg = nullptr;
+	int *d_jlen = nullptr, *d_jseg = nullptr, *d_jkeep = nullptr;
+	long long *d_jpsum = nullptr, *d_joff = nullptr, *d_jtotal = nullptr, *pin_jtotal = nullptr;
+	char *pin_jtext = nullptr;
+	std::vector<int> json_seg;
+	long long json_lines = 0;
+	bool queue_overflow_pending = false;
+	std::string json_buf;
+	size_t json_pos = 0;
+	bool json_overflow_pending = false;
 	// everything dalloc, halloc and new_event created: aisgpu_destroy releases these (the streams are destroyed one by one)
 	std::vector<void *> dev_mem, host_mem;
 	std::vector<cudaEvent_t> events;
@@ -1492,6 +1515,57 @@ void build_nmea(aisgpu_msg &m, int own_mmsi, int *seq_counter) {
 	}
 }
 
+const int kJsonBatch = 4096; // frames decoded per launch group
+
+// Drops the oldest unread lines beyond ring_cap (a caller that polls only frames does not let json_buf grow without bound).
+void json_trim(aisgpu_handle *h) {
+	const long long over = h->json_lines - h->ring_cap;
+	if (over <= 0) return;
+	for (long long k = 0; k < over; k++) {
+		const char *b = h->json_buf.data() + h->json_pos;
+		const char *e = (const char *)memchr(b, '\n', h->json_buf.size() - h->json_pos);
+		h->json_pos += (size_t)(e - b) + 1;
+	}
+	h->json_lines -= over;
+	h->json_overflow_pending = true;
+}
+
+// The full JSON lines of out_queue[q0, end) (the frames a drain just published) -> json_buf, on the device (be_json.cu), in batches
+// of kJsonBatch frames; a submit split over two batches carries the bytes its lines have used into the second.
+int json_decode(aisgpu_handle *h, size_t q0) {
+	const int n_all = (int)(h->out_queue.size() - q0);
+	if (n_all <= 0) return 0;
+	h->json_buf.erase(0, h->json_pos); // what has been read
+	h->json_pos = 0;
+	cudaStream_t st = h->json_stream;
+	long long carry = 0;
+	for (int b0 = 0; b0 < n_all; b0 += kJsonBatch) {
+		const int n = std::min(kJsonBatch, n_all - b0);
+		const aisgpu_msg *q = h->out_queue.data() + q0 + b0;
+		// submits are contiguous in out_queue: seg[i] = the first frame of frame i's submit within this batch
+		h->json_seg.resize((size_t)n);
+		for (int i = 0; i < n; i++) h->json_seg[i] = (i > 0 && q[i].chunk == q[i - 1].chunk) ? h->json_seg[i - 1] : i;
+		if (b0 == 0 || q[0].chunk != q[-1].chunk) carry = 0;
+		CU(cudaMemcpyAsync(h->d_jmsg, q, (size_t)n * sizeof(aisgpu_msg), cudaMemcpyHostToDevice, st));
+		CU(cudaMemcpyAsync(h->d_jseg, h->json_seg.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
+		CU(aj_launch(h->d_jmsg, n, h->d_jprefix, (int)h->json_prefix.size(), h->json_mode, h->json_station, h->d_jslots, h->json_slot,
+					 h->d_jlen, h->d_jseg, h->json_cap, carry, h->d_jpsum, h->d_joff, h->d_jkeep, h->d_jtotal, h->d_jtext, st));
+		CU(cudaMemcpyAsync(h->pin_jtotal, h->d_jtotal, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+		CU(cudaStreamSynchronize(st));
+		const long long total = h->pin_jtotal[0], kept_lines = h->pin_jtotal[1];
+		carry = h->pin_jtotal[2];
+		if (total > 0) {
+			CU(cudaMemcpyAsync(h->pin_jtext, h->d_jtext, (size_t)total, cudaMemcpyDeviceToHost, st));
+			CU(cudaStreamSynchronize(st));
+			h->json_buf.append(h->pin_jtext, (size_t)total);
+		}
+		h->json_lines += kept_lines;
+		if (kept_lines < n) h->json_overflow_pending = true; // lines that did not fit their submit's json_cap bytes
+	}
+	json_trim(h);
+	return 0;
+}
+
 // Copies the frames with tickets [a, b) to the end of h_ring; tickets at or above `limit` were dropped by the kernels.
 int fetch_frames(aisgpu_handle *h, unsigned long long a, unsigned long long b, unsigned long long limit) {
 	const unsigned long long hi = std::min(b, std::max(a, limit));
@@ -1563,6 +1637,11 @@ int drain_ring(aisgpu_handle *h, long long upto) {
 		if (a.blk != b.blk) return a.blk < b.blk; // Rotate sends whole blocks: A then B per block (DSP.cpp:312-313)
 		return a.row < b.row;
 	});
+	if (h->json_on && h->out_pos > 0) { // frames and lines are queued side by side: keep only what has not been read
+		h->out_queue.erase(h->out_queue.begin(), h->out_queue.begin() + (long)h->out_pos);
+		h->out_pos = 0;
+	}
+	const size_t q0 = h->out_queue.size();
 	for (const FrameRec &r : h->h_ring) {
 		h->counters[0]++;
 		aisgpu_msg m;
@@ -1583,6 +1662,13 @@ int drain_ring(aisgpu_handle *h, long long upto) {
 		h->counters[1]++;
 		h->counters[channel_of_row(h, r.row) ? 6 : 5]++;
 		h->out_queue.push_back(m);
+	}
+	if (!h->json_on) return 0;
+	if (int rc = json_decode(h, q0)) return rc;
+	// a caller that polls only lines: the frames it does not read are kept up to ring_cap
+	if ((long long)h->out_queue.size() > h->ring_cap) {
+		h->out_queue.erase(h->out_queue.begin(), h->out_queue.end() - h->ring_cap);
+		h->queue_overflow_pending = true;
 	}
 	return 0;
 }
@@ -1980,10 +2066,89 @@ int aisgpu_poll_upto(aisgpu_handle *h, int64_t ticket, aisgpu_msg *out, int max,
 		h->err = "frame ring overflow: frames were dropped (see counters[4]); raise aisgpu_config.max_frames or poll more often";
 		return AISGPU_EOVERFLOW;
 	}
+	if (h->queue_overflow_pending) {
+		h->queue_overflow_pending = false;
+		h->err = "frames were dropped from the host queue: with JSON enabled, more than max_frames frames were left unread";
+		return AISGPU_EOVERFLOW;
+	}
 	return 0;
 }
 
 int aisgpu_poll(aisgpu_handle *h, aisgpu_msg *out, int max, int *n) { return aisgpu_poll_upto(h, -1, out, max, n); }
+
+int aisgpu_json_enable(aisgpu_handle *h, const aisgpu_tag *tag, int max_bytes_per_submit) {
+	ENTER(h);
+	if (!tag || max_bytes_per_submit <= 0) {
+		h->err = "aisgpu_json_enable: bad argument";
+		return AISGPU_EINVAL;
+	}
+	if (h->counters[3] > 0 || h->json_on) {
+		h->err = h->json_on ? "aisgpu_json_enable: JSON is already enabled" : "aisgpu_json_enable: the engine has been submitted to";
+		return AISGPU_EINVAL;
+	}
+	h->json_prefix = aj_prefix(tag);
+	h->json_mode = tag->mode;
+	h->json_station = tag->station;
+	h->json_cap = max_bytes_per_submit;
+	// a line's slot: the prefix and the longest body, four fully escaped sentences (2.4 KB) plus the longest fields (1.3 KB)
+	h->json_slot = (int)((h->json_prefix.size() + 4096 + 15) / 16 * 16);
+	CU(cudaStreamCreateWithFlags(&h->json_stream, cudaStreamNonBlocking));
+	const size_t text = (size_t)kJsonBatch * h->json_slot;
+	if (int rc = dalloc(h, &h->d_jprefix, h->json_prefix.size() + 1)) return rc;
+	if (int rc = dalloc(h, &h->d_jtotal, 3)) return rc;
+	if (int rc = halloc(h, &h->pin_jtotal, 3)) return rc;
+	if (int rc = dalloc(h, &h->d_jmsg, kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jslots, text)) return rc;
+	if (int rc = dalloc(h, &h->d_jtext, text + kJsonBatch)) return rc; // a newline per line beyond its slot
+	if (int rc = halloc(h, &h->pin_jtext, text + kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jlen, kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jseg, kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jkeep, kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jpsum, kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_joff, kJsonBatch)) return rc;
+	CU(cudaMemcpy(h->d_jprefix, h->json_prefix.c_str(), h->json_prefix.size() + 1, cudaMemcpyHostToDevice));
+	h->json_on = true;
+	return 0;
+}
+
+int aisgpu_poll_json(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_lines) {
+	if (!n_bytes || !n_lines || (cap > 0 && !out)) return AISGPU_EINVAL;
+	ENTER(h);
+	if (!h->json_on) {
+		h->err = "aisgpu_poll_json: JSON is not enabled (aisgpu_json_enable)";
+		return AISGPU_EINVAL;
+	}
+	*n_bytes = 0;
+	*n_lines = 0;
+	if (h->json_pos >= h->json_buf.size())
+		if (int rc = drain_ring(h, (long long)ticket)) return rc;
+	size_t k = 0;
+	int lines = 0;
+	const char *b = h->json_buf.data();
+	while (h->json_pos + k < h->json_buf.size()) {
+		const char *s = b + h->json_pos + k;
+		const char *e = (const char *)memchr(s, '\n', h->json_buf.size() - h->json_pos - k);
+		const size_t l = (size_t)(e - s) + 1;
+		if (k + l > cap) break;
+		k += l;
+		lines++;
+	}
+	if (lines == 0 && h->json_pos < h->json_buf.size()) {
+		h->err = "aisgpu_poll_json: cap is smaller than the next line";
+		return AISGPU_EINVAL;
+	}
+	memcpy(out, b + h->json_pos, k);
+	h->json_pos += k;
+	h->json_lines -= lines;
+	*n_bytes = k;
+	*n_lines = lines;
+	if (h->json_overflow_pending) {
+		h->json_overflow_pending = false;
+		h->err = "JSON text overflow: lines were dropped; raise max_bytes_per_submit of aisgpu_json_enable";
+		return AISGPU_EOVERFLOW;
+	}
+	return 0;
+}
 
 int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, size_t dst_bytes, size_t *n_out) {
 	if (!h || !n_out || stream < 0 || stream >= h->cfg.n_streams || channel < 0 || channel > 9) return AISGPU_EINVAL;
@@ -2430,6 +2595,10 @@ void aisgpu_destroy(aisgpu_handle *h) {
 	if (h->copy_stream) cudaStreamSynchronize(h->copy_stream);
 	if (h->side_stream) cudaStreamSynchronize(h->side_stream);
 	if (h->dump_stream) cudaStreamSynchronize(h->dump_stream);
+	if (h->json_stream) {
+		cudaStreamSynchronize(h->json_stream);
+		cudaStreamDestroy(h->json_stream);
+	}
 	for (void *p : h->dev_mem) cudaFree(p);
 	for (void *p : h->host_mem) cudaFreeHost(p);
 	for (cudaEvent_t e : h->events) cudaEventDestroy(e);

@@ -32,6 +32,9 @@
 extern "C" {
 #endif
 
+/* 3 since the engine groups; later additions are new entry points only (the full AIS JSON: aisgpu_msg_json_full, aisgpu_json_enable,
+ * aisgpu_poll_json), so the number callers check against stays 3.  A caller that needs those entry points looks them up
+ * (dlsym) instead of relying on the number. */
 #define AISGPU_ABI_VERSION 3
 
 /* model kinds: the reference's "-m" numbers (Source/Application/Receiver.cpp:155-195) */
@@ -283,6 +286,38 @@ typedef struct aisgpu_tag {
  * "NMEA JSON" outputs, number formatting as JSON::Writer (Writer.h:174-218).  Returns the bytes written (no NUL is appended),
  * AISGPU_EOVERFLOW if cap is too small. Host-only. */
 int aisgpu_msg_json(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int cap);
+
+/* == the line JSON::Serializer(JSON_DICT_FULL) writes for AIS::JSONAIS::ProcessMsg(msg, tag) (Source/JSON/JSONAIS.cpp:1092-1533,
+ * Source/JSON/Writer.h): the full AIS JSON of -o 5, MSGFORMAT JSON_FULL and the HTTP / UDP / MQTT JSON outputs, decoded by the
+ * table interpreter the engine runs on the device (aisgpu_poll_json), built for the host.  From *tag it takes version, driver,
+ * hardware, mode (bit 0: signalpower / ppm from the aisgpu_msg unless 1024; bit 1: rxtime / rxuxtime from rxtime_us; bit 2: country
+ * and country_code of the MMSI's MID), toa_us (printed when non-zero), station (station_id when non-zero) and suffix (appended);
+ * status, ipv4, include_ssl and uuid are not part of this line.  The sentences under "nmea" are m's own.  Every message type and
+ * every application message (DAC, FI) of types 6, 8, 25 and 26 that the reference decodes into fields is decoded (ProcessMsg6Data /
+ * ProcessMsg8Data, JSONAIS.cpp:979-1044), repeated records included; any other (DAC, FI) is printed as "data", as the reference
+ * prints it.  Returns the bytes written (no NUL), AISGPU_EOVERFLOW if cap is too small, AISGPU_EINVAL for a NULL argument.
+ * Host-only. */
+int aisgpu_msg_json_full(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int cap);
+
+/* The full AIS JSON of every published frame, decoded on the GPU.  aisgpu_json_enable (before the first submit; once) fixes the tag
+ * every line is printed with (as for aisgpu_msg_json_full; suffix is not used) and max_bytes_per_submit, the text one submit's
+ * lines may take, newlines included.  From then on every poll of the frame ring -- aisgpu_poll, aisgpu_poll_upto, aisgpu_poll_json
+ * and the feeders' -- decodes the frames it publishes on the device: one upload of those frames and three kernels on a stream of
+ * its own, never the front end or the demodulation kernels, so frames, taps and counters do not change.  A group member decodes
+ * its own frames (enable it on the member).
+ *
+ * aisgpu_poll_json is aisgpu_poll_upto for the lines: it drains the frames of the submits up to ticket if no line is waiting, and
+ * copies whole lines, each ended by '\n', in the order aisgpu_poll returns the frames, until the next would pass cap; *n_bytes and
+ * *n_lines receive what was written.  Call it again until *n_lines == 0.  Line i is frame i: the frames and the lines a poll
+ * publishes are queued side by side, and each queue is read by its own call (aisgpu_poll* / aisgpu_poll_json), so a caller may
+ * take both, or only one of them.  Neither queue keeps more than max_frames (aisgpu_config) unread entries: beyond that the oldest
+ * are dropped, and the next poll of that kind returns AISGPU_EOVERFLOW with what survived -- a caller that takes only lines (or
+ * only frames) thus holds at most max_frames of the other in host memory.  Lines past a submit's max_bytes_per_submit are dropped,
+ * later lines of that submit too, and the next aisgpu_poll_json returns AISGPU_EOVERFLOW with the lines that survived, as the frame
+ * ring does.  AISGPU_EINVAL when JSON is not enabled, or when cap is smaller than the next line.  The engine allocates, at enable,
+ * about 8.6 KB of device memory and 4.3 KB of pinned host memory per frame of a 4096-frame decode batch. */
+int aisgpu_json_enable(aisgpu_handle *h, const aisgpu_tag *tag, int max_bytes_per_submit);
+int aisgpu_poll_json(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_lines);
 
 /* == AIS::Message::getBinaryNMEA(out, tag, crc) (Message.cpp:277-396): 0xAC 0x00 framed, byte-stuffed binary record with an
  * optional CRC-16 (Helper.cpp:42-57).  Returns the bytes written, 0 when the reference would emit nothing. Host-only. */
