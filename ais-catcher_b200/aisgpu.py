@@ -25,9 +25,20 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_poll_upto", "aisgpu_nccl_unique_id", "aisgpu_comm_init", "aisgpu_allreduce_counts",
            "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
            "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files",
-           "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json"]
+           "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json", "aisgpu_msg_format", "aisgpu_lines_enable",
+           "aisgpu_poll_lines"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
+# message formats: positions in the reference's enum class MessageFormat (MSGFORMAT of its outputs); include/aisgpu.h describes each record
+(MSGFORMAT_NMEA, MSGFORMAT_NMEA_TAG, MSGFORMAT_COMMUNITY_HUB, MSGFORMAT_BINARY_NMEA, MSGFORMAT_FULL, MSGFORMAT_JSON_NMEA,
+ MSGFORMAT_JSON_SPARSE, MSGFORMAT_JSON_FULL, MSGFORMAT_JSON_ANNOTATED) = range(1, 10)
+MSGFORMATS = {"NMEA": 1, "NMEA_TAG": 2, "COMMUNITY_HUB": 3, "BINARY_NMEA": 4, "FULL": 5, "JSON_NMEA": 6, "JSON_SPARSE": 7,
+              "JSON_FULL": 8, "JSON_ANNOTATED": 9}
+
+
+class FormatState(C.Structure):
+    """aisgpu_format_state: the engine's counters for msg_format (records formatted, multi-sentence frames among them)."""
+    _fields_ = [("records", C.c_int64), ("groups", C.c_int64)]
 
 
 class Config(C.Structure):
@@ -130,6 +141,11 @@ def load():
         lib.aisgpu_msg_json_full.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
         lib.aisgpu_json_enable.argtypes = [C.c_void_p, C.POINTER(TagStruct), C.c_int]
         lib.aisgpu_poll_json.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int)]
+    if hasattr(lib, "aisgpu_msg_format"):  # absent from libraries built before the output records (AISGPU_LIB)
+        lib.aisgpu_msg_format.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_int, C.POINTER(FormatState), C.c_char_p,
+                                          C.c_int]
+        lib.aisgpu_lines_enable.argtypes = [C.c_void_p, C.c_int, C.POINTER(TagStruct), C.c_int]
+        lib.aisgpu_poll_lines.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int)]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -219,6 +235,18 @@ def msg_json_full(m, tag, cap=65536):
     n = load().aisgpu_msg_json_full(C.byref(m), C.byref(tag), buf, cap)
     if n < 0:
         raise AisGpuError("aisgpu_msg_json_full rc=%d" % n)
+    return buf.raw[:n]
+
+
+def msg_format(m, tag, fmt, state=None, cap=1 << 16):
+    """Host-only: aisgpu_msg_format, the record of m (make_msg or a polled Msg) in MSGFORMAT fmt (1..9) with tag -> bytes.
+    state: a FormatState, advanced as the engine advances its counters (None: both 0)."""
+    if isinstance(m, Msg):
+        m = msg_struct(m)
+    buf = C.create_string_buffer(cap)
+    n = load().aisgpu_msg_format(C.byref(m), C.byref(tag), int(fmt), C.byref(state) if state is not None else None, buf, cap)
+    if n < 0:
+        raise AisGpuError("aisgpu_msg_format rc=%d" % n)
     return buf.raw[:n]
 
 
@@ -448,6 +476,27 @@ class Engine:
                 break
             out.extend(buf.raw[:nb.value].decode("utf-8", "surrogateescape").split("\n")[:-1])
         return out
+
+    def lines_enable(self, fmt, tag=None, max_bytes_per_submit=1 << 24):
+        """aisgpu_lines_enable: from the first submit on, every polled frame is also formatted on the GPU as its record in
+        MSGFORMAT fmt (1..9) with tag (make_tag(); default: make_tag(); suffix None: CR LF), at most max_bytes_per_submit bytes of
+        records per submit."""
+        self._json_tag = tag if tag is not None else make_tag()
+        self._chk(self.lib.aisgpu_lines_enable(self.h, int(fmt), C.byref(self._json_tag), int(max_bytes_per_submit)))
+
+    def poll_lines(self, ticket=None, cap=1 << 20):
+        """aisgpu_poll_lines: (bytes, number of records) of the frames of the submits up to ticket (None: all), in frame order."""
+        t = -1 if ticket is None else int(ticket)
+        buf = C.create_string_buffer(cap)
+        nb, nr = C.c_size_t(0), C.c_int(0)
+        out, n = [], 0
+        while True:
+            self._chk(self.lib.aisgpu_poll_lines(self.h, t, buf, cap, C.byref(nb), C.byref(nr)))
+            if nr.value == 0:
+                break
+            out.append(buf.raw[:nb.value])
+            n += nr.value
+        return b"".join(out), n
 
     def poll(self, batch=256):
         out = []

@@ -289,24 +289,27 @@ struct aisgpu_handle {
 	std::deque<DumpPending> dump_pending; // slots copied or being copied, not yet written, in submit order
 	int dump_slot = -1;                   // the submit being enqueued: its slot (-1: no export), row length and columns exported so far
 	long long dump_n = 0, dump_off = 0;
-	// The full AIS JSON (aisgpu_json_enable).  Every drain of the frame ring uploads the frames it publishes to d_jmsg, kJsonBatch
-	// at a time, and decodes them on json_stream (be_json.cu: a line per frame into its slot, the placement within json_cap bytes
-	// per submit, the packed text); the text comes back through pin_jtext and is appended to json_buf, which aisgpu_poll_json hands
-	// out from json_pos on.  Frames and lines are queued side by side and each is read by its own poll; neither queue keeps more
-	// than ring_cap unread entries (json_lines counts the unread lines): the oldest are dropped and the next poll of that kind
-	// returns AISGPU_EOVERFLOW.  Nothing of this exists while JSON has not been enabled.
-	bool json_on = false;
-	int json_mode = 0, json_station = 0, json_slot = 0;
-	long long json_cap = 0;
-	std::string json_prefix;
+	// The output records (aisgpu_lines_enable; aisgpu_json_enable is JSON_FULL with suffix "\n").  Every drain of the frame ring
+	// uploads the frames it publishes to d_jmsg, kJsonBatch at a time, and formats them on json_stream (be_json.cu: the NMEA_TAG
+	// group counts, a record per frame into its slot, the placement within json_cap bytes per submit, the packed text); the text
+	// comes back through pin_jtext and is appended to json_buf, which aisgpu_poll_lines / aisgpu_poll_json hand out from json_pos
+	// on, and the kept records' lengths (pin_jkeep) to rec_len.  fmt_records / fmt_groups are the engine's counters (frames
+	// published, multi-sentence ones among them), carried from batch to batch.  Frames and records are queued side by side and
+	// each is read by its own poll; neither queue keeps more than ring_cap unread entries: the oldest are dropped and the next poll
+	// of that kind returns AISGPU_EOVERFLOW.  Nothing of this exists while no format has been enabled.
+	bool json_on = false, json_api = false;
+	int fmt = 0, json_slot = 0, rec_cap = 0;
+	long long json_cap = 0, fmt_records = 0, fmt_groups = 0;
+	std::string fmt_strings; // the tag's strings: hardware, uuid, suffix and the full-JSON prefix, each NUL-terminated
+	FmtCtx *d_fctx = nullptr;
 	cudaStream_t json_stream = nullptr;
-	char *d_jprefix = nullptr, *d_jslots = nullptr, *d_jtext = nullptr;
+	char *d_jstrings = nullptr, *d_jslots = nullptr, *d_jtext = nullptr;
 	aisgpu_msg *d_jmsg = nullptr;
-	int *d_jlen = nullptr, *d_jseg = nullptr, *d_jkeep = nullptr;
-	long long *d_jpsum = nullptr, *d_joff = nullptr, *d_jtotal = nullptr, *pin_jtotal = nullptr;
+	int *d_jlen = nullptr, *d_jseg = nullptr, *d_jkeep = nullptr, *pin_jkeep = nullptr;
+	long long *d_jpsum = nullptr, *d_joff = nullptr, *d_jtotal = nullptr, *pin_jtotal = nullptr, *d_jgroups = nullptr;
 	char *pin_jtext = nullptr;
 	std::vector<int> json_seg;
-	long long json_lines = 0;
+	std::deque<int> rec_len; // the unread records' lengths
 	bool queue_overflow_pending = false;
 	std::string json_buf;
 	size_t json_pos = 0;
@@ -1517,21 +1520,19 @@ void build_nmea(aisgpu_msg &m, int own_mmsi, int *seq_counter) {
 
 const int kJsonBatch = 4096; // frames decoded per launch group
 
-// Drops the oldest unread lines beyond ring_cap (a caller that polls only frames does not let json_buf grow without bound).
+// Drops the oldest unread records beyond ring_cap (a caller that polls only frames does not let json_buf grow without bound).
 void json_trim(aisgpu_handle *h) {
-	const long long over = h->json_lines - h->ring_cap;
-	if (over <= 0) return;
-	for (long long k = 0; k < over; k++) {
-		const char *b = h->json_buf.data() + h->json_pos;
-		const char *e = (const char *)memchr(b, '\n', h->json_buf.size() - h->json_pos);
-		h->json_pos += (size_t)(e - b) + 1;
+	if ((long long)h->rec_len.size() <= h->ring_cap) return;
+	while ((long long)h->rec_len.size() > h->ring_cap) {
+		h->json_pos += (size_t)h->rec_len.front();
+		h->rec_len.pop_front();
 	}
-	h->json_lines -= over;
 	h->json_overflow_pending = true;
 }
 
-// The full JSON lines of out_queue[q0, end) (the frames a drain just published) -> json_buf, on the device (be_json.cu), in batches
-// of kJsonBatch frames; a submit split over two batches carries the bytes its lines have used into the second.
+// The records of out_queue[q0, end) (the frames a drain just published) -> json_buf, on the device (be_json.cu), in batches of
+// kJsonBatch frames; a submit split over two batches carries the bytes its records have used into the second, and every batch
+// carries the engine's counters into the next.
 int json_decode(aisgpu_handle *h, size_t q0) {
 	const int n_all = (int)(h->out_queue.size() - q0);
 	if (n_all <= 0) return 0;
@@ -1548,19 +1549,23 @@ int json_decode(aisgpu_handle *h, size_t q0) {
 		if (b0 == 0 || q[0].chunk != q[-1].chunk) carry = 0;
 		CU(cudaMemcpyAsync(h->d_jmsg, q, (size_t)n * sizeof(aisgpu_msg), cudaMemcpyHostToDevice, st));
 		CU(cudaMemcpyAsync(h->d_jseg, h->json_seg.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-		CU(aj_launch(h->d_jmsg, n, h->d_jprefix, (int)h->json_prefix.size(), h->json_mode, h->json_station, h->d_jslots, h->json_slot,
-					 h->d_jlen, h->d_jseg, h->json_cap, carry, h->d_jpsum, h->d_joff, h->d_jkeep, h->d_jtotal, h->d_jtext, st));
-		CU(cudaMemcpyAsync(h->pin_jtotal, h->d_jtotal, 3 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+		CU(fmt_launch(h->d_jmsg, n, h->d_fctx, h->fmt_records, h->fmt_groups, h->d_jgroups, h->d_jslots, h->json_slot, h->rec_cap,
+					  h->d_jlen, h->d_jseg, h->json_cap, carry, h->d_jpsum, h->d_joff, h->d_jkeep, h->d_jtotal, h->d_jtext, st));
+		CU(cudaMemcpyAsync(h->pin_jtotal, h->d_jtotal, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+		CU(cudaMemcpyAsync(h->pin_jkeep, h->d_jkeep, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
 		CU(cudaStreamSynchronize(st));
-		const long long total = h->pin_jtotal[0], kept_lines = h->pin_jtotal[1];
+		const long long total = h->pin_jtotal[0], kept = h->pin_jtotal[1];
 		carry = h->pin_jtotal[2];
+		h->fmt_records += n;
+		h->fmt_groups += h->pin_jtotal[3];
 		if (total > 0) {
 			CU(cudaMemcpyAsync(h->pin_jtext, h->d_jtext, (size_t)total, cudaMemcpyDeviceToHost, st));
 			CU(cudaStreamSynchronize(st));
 			h->json_buf.append(h->pin_jtext, (size_t)total);
 		}
-		h->json_lines += kept_lines;
-		if (kept_lines < n) h->json_overflow_pending = true; // lines that did not fit their submit's json_cap bytes
+		for (int i = 0; i < n; i++)
+			if (h->pin_jkeep[i] >= 0) h->rec_len.push_back(h->pin_jkeep[i]);
+		if (kept < n) h->json_overflow_pending = true; // records that did not fit their submit's json_cap bytes
 	}
 	json_trim(h);
 	return 0;
@@ -2076,78 +2081,120 @@ int aisgpu_poll_upto(aisgpu_handle *h, int64_t ticket, aisgpu_msg *out, int max,
 
 int aisgpu_poll(aisgpu_handle *h, aisgpu_msg *out, int max, int *n) { return aisgpu_poll_upto(h, -1, out, max, n); }
 
-int aisgpu_json_enable(aisgpu_handle *h, const aisgpu_tag *tag, int max_bytes_per_submit) {
+namespace {
+
+// aisgpu_lines_enable and aisgpu_json_enable (who: the entry point, for the messages)
+int lines_enable(aisgpu_handle *h, int fmt, const aisgpu_tag *tag, const char *suffix, int max_bytes_per_submit, bool json_api,
+				 const char *who) {
 	ENTER(h);
-	if (!tag || max_bytes_per_submit <= 0) {
-		h->err = "aisgpu_json_enable: bad argument";
+	if (!tag || max_bytes_per_submit <= 0 || fmt < AISGPU_MSGFORMAT_NMEA || fmt > AISGPU_MSGFORMAT_JSON_ANNOTATED) {
+		h->err = std::string(who) + ": bad argument";
 		return AISGPU_EINVAL;
 	}
 	if (h->counters[3] > 0 || h->json_on) {
-		h->err = h->json_on ? "aisgpu_json_enable: JSON is already enabled" : "aisgpu_json_enable: the engine has been submitted to";
+		h->err = std::string(who) + (h->json_on ? ": a format is already enabled" : ": the engine has been submitted to");
 		return AISGPU_EINVAL;
 	}
-	h->json_prefix = aj_prefix(tag);
-	h->json_mode = tag->mode;
-	h->json_station = tag->station;
+	const char *hw = tag->hardware ? tag->hardware : "", *uuid = tag->uuid ? tag->uuid : "";
+	const std::string prefix = aj_prefix(tag);
+	h->fmt_strings = std::string(hw) + '\0' + uuid + '\0' + suffix + '\0' + prefix + '\0';
+	h->fmt = fmt;
+	h->json_api = json_api;
 	h->json_cap = max_bytes_per_submit;
-	// a line's slot: the prefix and the longest body, four fully escaped sentences (2.4 KB) plus the longest fields (1.3 KB)
-	h->json_slot = (int)((h->json_prefix.size() + 4096 + 15) / 16 * 16);
+	// a record's room: the longest record of its format with the tag's strings (the hardware name escaped, uuid and suffix once per
+	// sentence) -- four fully escaped sentences (2.4 KB) plus the longest fields (1.3 KB) after the full-JSON prefix, and for
+	// JSON_ANNOTATED their units and descriptions besides; JSON_SPARSE and JSON_ANNOTATED add a scratch full line to the slot
+	const size_t strs = prefix.size() + strlen(hw) * 6 + (strlen(uuid) + strlen(suffix)) * 4;
+	const bool rewritten = fmt == AISGPU_MSGFORMAT_JSON_SPARSE || fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED;
+	h->rec_cap = (int)((strs + (fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED ? 20480 : 4096) + 15) / 16 * 16);
+	h->json_slot = h->rec_cap + (rewritten ? (int)((prefix.size() + 4096 + 15) / 16 * 16) : 0);
 	CU(cudaStreamCreateWithFlags(&h->json_stream, cudaStreamNonBlocking));
-	const size_t text = (size_t)kJsonBatch * h->json_slot;
-	if (int rc = dalloc(h, &h->d_jprefix, h->json_prefix.size() + 1)) return rc;
-	if (int rc = dalloc(h, &h->d_jtotal, 3)) return rc;
-	if (int rc = halloc(h, &h->pin_jtotal, 3)) return rc;
+	const size_t text = (size_t)kJsonBatch * h->rec_cap;
+	if (int rc = dalloc(h, &h->d_jstrings, h->fmt_strings.size())) return rc;
+	if (int rc = dalloc(h, &h->d_fctx, 1)) return rc;
+	if (int rc = dalloc(h, &h->d_jtotal, 4)) return rc;
+	if (int rc = halloc(h, &h->pin_jtotal, 4)) return rc;
 	if (int rc = dalloc(h, &h->d_jmsg, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_jslots, text)) return rc;
-	if (int rc = dalloc(h, &h->d_jtext, text + kJsonBatch)) return rc; // a newline per line beyond its slot
-	if (int rc = halloc(h, &h->pin_jtext, text + kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jslots, (size_t)kJsonBatch * h->json_slot)) return rc;
+	if (int rc = dalloc(h, &h->d_jtext, text)) return rc;
+	if (int rc = halloc(h, &h->pin_jtext, text)) return rc;
 	if (int rc = dalloc(h, &h->d_jlen, kJsonBatch)) return rc;
 	if (int rc = dalloc(h, &h->d_jseg, kJsonBatch)) return rc;
 	if (int rc = dalloc(h, &h->d_jkeep, kJsonBatch)) return rc;
+	if (int rc = halloc(h, &h->pin_jkeep, kJsonBatch)) return rc;
+	if (int rc = dalloc(h, &h->d_jgroups, kJsonBatch)) return rc;
 	if (int rc = dalloc(h, &h->d_jpsum, kJsonBatch)) return rc;
 	if (int rc = dalloc(h, &h->d_joff, kJsonBatch)) return rc;
-	CU(cudaMemcpy(h->d_jprefix, h->json_prefix.c_str(), h->json_prefix.size() + 1, cudaMemcpyHostToDevice));
+	// dalloc zeroes each buffer on h->stream: the strings and the context are written after that, not under it
+	CU(cudaStreamSynchronize(h->stream));
+	CU(cudaMemcpy(h->d_jstrings, h->fmt_strings.data(), h->fmt_strings.size(), cudaMemcpyHostToDevice));
+	FmtCtx c = fmt_ctx(tag, fmt, suffix, prefix);
+	c.hardware = h->d_jstrings;
+	c.uuid = c.hardware + strlen(hw) + 1;
+	c.suffix = c.uuid + strlen(uuid) + 1;
+	c.prefix = c.suffix + strlen(suffix) + 1;
+	CU(cudaMemcpy(h->d_fctx, &c, sizeof(c), cudaMemcpyHostToDevice));
 	h->json_on = true;
 	return 0;
+}
+
+// aisgpu_poll_lines and aisgpu_poll_json: whole records from the queue until the next would pass cap
+int poll_records(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_records, const char *who) {
+	*n_bytes = 0;
+	*n_records = 0;
+	if (h->rec_len.empty())
+		if (int rc = drain_ring(h, (long long)ticket)) return rc;
+	size_t k = 0;
+	int recs = 0;
+	while (recs < (int)h->rec_len.size() && k + (size_t)h->rec_len[recs] <= cap) k += (size_t)h->rec_len[recs++];
+	if (recs == 0 && !h->rec_len.empty()) {
+		h->err = std::string(who) + (h->json_api ? ": cap is smaller than the next line" : ": cap is smaller than the next record");
+		return AISGPU_EINVAL;
+	}
+	if (k) memcpy(out, h->json_buf.data() + h->json_pos, k);
+	h->json_pos += k;
+	h->rec_len.erase(h->rec_len.begin(), h->rec_len.begin() + recs);
+	*n_bytes = k;
+	*n_records = recs;
+	if (h->json_overflow_pending) {
+		h->json_overflow_pending = false;
+		h->err = h->json_api ? "JSON text overflow: lines were dropped; raise max_bytes_per_submit of aisgpu_json_enable"
+							 : "record overflow: records were dropped; raise max_bytes_per_submit of aisgpu_lines_enable";
+		return AISGPU_EOVERFLOW;
+	}
+	return 0;
+}
+
+} // namespace
+
+int aisgpu_json_enable(aisgpu_handle *h, const aisgpu_tag *tag, int max_bytes_per_submit) {
+	return lines_enable(h, AISGPU_MSGFORMAT_JSON_FULL, tag, "\n", max_bytes_per_submit, true, "aisgpu_json_enable");
+}
+
+int aisgpu_lines_enable(aisgpu_handle *h, int msgformat, const aisgpu_tag *tag, int max_bytes_per_submit) {
+	return lines_enable(h, msgformat, tag, tag && tag->suffix ? tag->suffix : "\r\n", max_bytes_per_submit, false,
+						"aisgpu_lines_enable");
 }
 
 int aisgpu_poll_json(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_lines) {
 	if (!n_bytes || !n_lines || (cap > 0 && !out)) return AISGPU_EINVAL;
 	ENTER(h);
+	if (!h->json_api) {
+		h->err = h->json_on ? "aisgpu_poll_json: the engine formats another message format (aisgpu_poll_lines)"
+							: "aisgpu_poll_json: JSON is not enabled (aisgpu_json_enable)";
+		return AISGPU_EINVAL;
+	}
+	return poll_records(h, ticket, out, cap, n_bytes, n_lines, "aisgpu_poll_json");
+}
+
+int aisgpu_poll_lines(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_records) {
+	if (!n_bytes || !n_records || (cap > 0 && !out)) return AISGPU_EINVAL;
+	ENTER(h);
 	if (!h->json_on) {
-		h->err = "aisgpu_poll_json: JSON is not enabled (aisgpu_json_enable)";
+		h->err = "aisgpu_poll_lines: no format is enabled (aisgpu_lines_enable)";
 		return AISGPU_EINVAL;
 	}
-	*n_bytes = 0;
-	*n_lines = 0;
-	if (h->json_pos >= h->json_buf.size())
-		if (int rc = drain_ring(h, (long long)ticket)) return rc;
-	size_t k = 0;
-	int lines = 0;
-	const char *b = h->json_buf.data();
-	while (h->json_pos + k < h->json_buf.size()) {
-		const char *s = b + h->json_pos + k;
-		const char *e = (const char *)memchr(s, '\n', h->json_buf.size() - h->json_pos - k);
-		const size_t l = (size_t)(e - s) + 1;
-		if (k + l > cap) break;
-		k += l;
-		lines++;
-	}
-	if (lines == 0 && h->json_pos < h->json_buf.size()) {
-		h->err = "aisgpu_poll_json: cap is smaller than the next line";
-		return AISGPU_EINVAL;
-	}
-	memcpy(out, b + h->json_pos, k);
-	h->json_pos += k;
-	h->json_lines -= lines;
-	*n_bytes = k;
-	*n_lines = lines;
-	if (h->json_overflow_pending) {
-		h->json_overflow_pending = false;
-		h->err = "JSON text overflow: lines were dropped; raise max_bytes_per_submit of aisgpu_json_enable";
-		return AISGPU_EOVERFLOW;
-	}
-	return 0;
+	return poll_records(h, ticket, out, cap, n_bytes, n_records, "aisgpu_poll_lines");
 }
 
 int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, size_t dst_bytes, size_t *n_out) {

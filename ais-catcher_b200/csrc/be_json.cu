@@ -1,6 +1,10 @@
-// The full AIS JSON of a frame -- what the reference's JSONAIS::ProcessMsg builds and JSON::Serializer(JSON_DICT_FULL) writes for
-// -o 5, MSGFORMAT JSON_FULL and the HTTP / UDP / MQTT JSON outputs -- decoded by one table interpreter that is compiled twice: on
-// the device (one thread per published frame, aisgpu_poll_json) and on the host (aisgpu_msg_json_full).
+// The record of a frame in every message format of the reference's outputs (MSGFORMAT, OutputMessage::formatInto) -- NMEA,
+// NMEA_TAG, COMMUNITY_HUB, BINARY_NMEA, FULL, JSON_NMEA, and the full AIS JSON that JSONAIS::ProcessMsg builds, written by
+// JSON::Serializer in the full (JSON_FULL: -o 5 and the HTTP / UDP / MQTT JSON outputs) or sparse dictionary (JSON_SPARSE) or
+// annotated (JSON_ANNOTATED) -- by one formatter around one table interpreter.  The interpreter is written against a writer: the
+// engine runs it on the device with the plain full-dictionary writer Out (one thread per published frame, aisgpu_poll_json); the
+// host runs it with Out (aisgpu_msg_json_full) and with the dictionary-aware DOut, inside the record formatter (aisgpu_msg_format and
+// the egress formatters aisgpu_msg_json / aisgpu_msg_binary).
 //
 // A message type is a program of field operations (U / UL / SL / E / B / TURN / text / timestamp / ETA / data / radio) in
 // constant memory; the layouts with control flow (types 22, 24, 25, 26 and the application messages of 6 and 8) pick programs in
@@ -15,12 +19,17 @@
 // as "data" ("<bits>:<hex>"), as the reference does.
 
 #include "be_json.h"
+#include "fmt_text.h"
 #include "json_text.h"
 
 #include <cub/block/block_scan.cuh>
 #include <math.h>
 #include <stdint.h>
 #include <string.h>
+
+#include <string>
+#include <vector>
+
 
 namespace {
 
@@ -71,7 +80,8 @@ namespace {
 	X(end_time) X(start_lon) X(start_lat) X(end_lon) X(end_lat) X(emma_warning_type) X(min_value) X(max_value) X(emma_severity)    \
 	X(wind_direction) X(gauge1_id) X(gauge1_level) X(gauge2_id) X(gauge2_level) X(gauge3_id) X(gauge3_level) X(gauge4_id)          \
 	X(gauge4_level) X(signal_form) X(signal_orientation) X(signal_impact) X(signal_status) X(planned_speed) X(steering_mode)       \
-	X(last_port) X(next_port) X(second_port) X(tidal) X(traffic_signal) X(next_signal) X(targets)
+	X(last_port) X(next_port) X(second_port) X(tidal) X(traffic_signal) X(next_signal) X(targets) X(class) X(device) X(driver)     \
+	X(hardware) X(rxtime) X(rxuxtime) X(toa) X(scaled) X(channel) X(nmea) X(signalpower) X(ppm)
 
 enum Key : uint16_t {
 #define X(n) K_##n,
@@ -122,6 +132,30 @@ AJ_TABLE(uint16_t, t_cname, AJ_COUNTRY_NAME_N, AJ_COUNTRY_NAME_INIT)
 AJ_TABLE(uint16_t, t_ccode, AJ_COUNTRY_CODE_N, AJ_COUNTRY_CODE_INIT)
 
 enum TextTab : uint8_t { TT_NONE, TT_NAV, TT_EPFD, TT_SHIP, TT_AID };
+
+// ---- the sparse names and the annotations (fmt_text.h, generated from the reference's output), in global memory ----
+#ifdef __CUDA_ARCH__
+#define AF_TAB(name) d_##name
+#else
+#define AF_TAB(name) h_##name
+#endif
+#define AF_TABLE(type, name, n, init)           \
+	static const type h_##name[n] = init;       \
+	__device__ const type d_##name[n] = init;
+#define NO 0xFFFFFFFFu
+static_assert(AF_KEY_N == K_COUNT, "fmt_text.h is generated from this file's key list: run tools/gen_fmt_text.py");
+struct AfBlob {
+	char s[AF_BLOB_SIZE + 1];
+};
+AF_TABLE(AfBlob, af_blob, 1, { { AF_BLOB } })
+AF_TABLE(uint32_t, af_sparse, AF_KEY_N, AF_SPARSE_INIT)
+AF_TABLE(uint32_t, af_unit, AF_KEY_N, AF_UNIT_INIT)
+AF_TABLE(uint32_t, af_desc, AF_KEY_N, AF_DESC_INIT)
+AF_TABLE(int16_t, af_lut, AF_KEY_N, AF_LUT_INIT)
+AF_TABLE(int, af_lut_at, AF_NLUT, AF_LUT_AT_INIT)
+AF_TABLE(int, af_lut_n, AF_NLUT, AF_LUT_N_INIT)
+AF_TABLE(uint32_t, af_lut_text, AF_LUT_TEXT_N, AF_LUT_TEXT_INIT)
+#undef NO
 
 // ---- field operations ----
 enum OpCode : uint8_t {
@@ -1166,7 +1200,440 @@ __host__ __device__ void body(Out &o, const Msg &m, const aisgpu_msg *src, int m
 	}
 }
 
-// one line: prefix, body, '}'; its length, or -2 when it does not fit in cap
+// Message::getRxTime / Convert::toTimeStr: YYYYMMDDHHMMSS (UTC) of the whole seconds, times before the epoch as the epoch
+__host__ __device__ void put_rxtime(Out &o, long long us) {
+	long long t = us / 1000000;
+	if (t < 0) t = 0;
+	const int sec = (int)(t % 60), mn = (int)(t / 60 % 60), hr = (int)(t / 3600 % 24);
+	const int z = (int)(t / 86400) + 719468, era = (z >= 0 ? z : z - 146096) / 146097;
+	const unsigned doe = (unsigned)(z - era * 146097), yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
+	const unsigned doy = doe - (365 * yoe + yoe / 4 - yoe / 100), mp = (5 * doy + 2) / 153;
+	const int day = (int)(doy - (153 * mp + 2) / 5 + 1), mon = (int)(mp + (mp < 10 ? 3 : -9));
+	const int year = (int)yoe + era * 400 + (mon <= 2);
+	const int parts[7] = { year / 100, year % 100, mon, day, hr, mn, sec };
+	for (int v : parts) put2(o, (unsigned)v);
+}
+
+// printf("%g", (double)f) as glibc prints it: the exact binary value rounded to six significant digits, ties to even; exponent
+// form when the decimal exponent after that rounding is below -4 or at least 6; trailing zeros trimmed.  The value is m * 2^e
+// with a 24-bit m; it is written as the integer M = m * 2^e (e >= 0) or m * 5^-e (e < 0, the decimal point -e digits from the
+// right), at most 371 bits, whose decimal digits give the rounding exactly.
+__host__ __device__ void put_g(Out &o, float f) {
+	uint32_t b;
+	memcpy(&b, &f, 4);
+	const int bexp = (int)((b >> 23) & 0xFF);
+	uint32_t man = b & 0x7FFFFF;
+	if (b >> 31) o.ch('-');
+	if (bexp == 0xFF) {
+		o.cstr(man ? "nan" : "inf");
+		return;
+	}
+	if (bexp == 0 && man == 0) {
+		o.ch('0');
+		return;
+	}
+	int e2 = -149;
+	if (bexp) {
+		man |= 0x800000;
+		e2 = bexp - 150;
+	}
+	uint32_t L[12];
+	int nl = 1;
+	L[0] = man;
+	auto mul = [&](uint32_t k) {
+		unsigned long long c = 0;
+		for (int i = 0; i < nl; i++) {
+			c += (unsigned long long)L[i] * k;
+			L[i] = (uint32_t)c;
+			c >>= 32;
+		}
+		if (c) L[nl++] = (uint32_t)c;
+	};
+	int q = 0; // the value is M * 10^q
+	if (e2 >= 0)
+		for (int k = e2; k > 0; k -= 31) mul(1u << (k < 31 ? k : 31));
+	else {
+		for (int k = -e2; k > 0; k -= 13) {
+			uint32_t p5 = 1;
+			for (int j = 0; j < (k < 13 ? k : 13); j++) p5 *= 5;
+			mul(p5);
+		}
+		q = e2;
+	}
+	char dg[120]; // M's decimal digits, least significant first
+	int nd = 0;
+	while (nl > 0) {
+		unsigned long long r = 0;
+		for (int i = nl - 1; i >= 0; i--) {
+			const unsigned long long cur = (r << 32) | L[i];
+			L[i] = (uint32_t)(cur / 1000000000u);
+			r = cur % 1000000000u;
+		}
+		while (nl > 0 && L[nl - 1] == 0) nl--;
+		for (int j = 0; j < 9 && (nl > 0 || r > 0); j++) {
+			dg[nd++] = (char)(r % 10);
+			r /= 10;
+		}
+	}
+	int E = nd - 1 + q; // decimal exponent of the leading digit
+	long K = 0;          // the six significant digits
+	for (int j = 0; j < 6; j++) K = K * 10 + (j < nd ? dg[nd - 1 - j] : 0);
+	if (nd > 6) {
+		const int d6 = dg[nd - 7];
+		bool rest = false;
+		for (int j = 0; j < nd - 7; j++) rest |= dg[j] != 0;
+		if (d6 > 5 || (d6 == 5 && (rest || (K & 1)))) K++;
+		if (K == 1000000) {
+			K = 100000;
+			E++;
+		}
+	}
+	char k6[6];
+	for (int j = 5; j >= 0; j--) {
+		k6[j] = (char)('0' + K % 10);
+		K /= 10;
+	}
+	int last = 5;
+	while (last > 0 && k6[last] == '0') last--;
+	if (E < -4 || E >= 6) {
+		o.ch(k6[0]);
+		if (last > 0) {
+			o.ch('.');
+			o.raw(k6 + 1, last);
+		}
+		o.ch('e');
+		o.ch(E < 0 ? '-' : '+');
+		const int a = E < 0 ? -E : E;
+		if (a >= 100) o.ch((char)('0' + a / 100));
+		put2(o, (unsigned)(a % 100));
+	}
+	else if (E >= 0) {
+		o.raw(k6, E + 1);
+		if (last > E) {
+			o.ch('.');
+			o.raw(k6 + E + 1, last - E);
+		}
+	}
+	else {
+		o.raw("0.", 2);
+		for (int j = 0; j < -E - 1; j++) o.ch('0');
+		o.raw(k6, last + 1);
+	}
+}
+
+__host__ __device__ int n_sent(const aisgpu_msg *src) { return src->n_sentences < 0 ? 0 : (src->n_sentences > 4 ? 4 : src->n_sentences); }
+__host__ __device__ int sent_len(const aisgpu_msg *src, int i) {
+	const int l = src->nmea_len[i];
+	return l < 0 ? 0 : (l > 100 ? 100 : l);
+}
+
+// ---- the sparse and the annotated JSON: the full line rewritten member by member ----
+// Every member of the full line is a key of AJ_KEYS; a key is found by its name through an open-addressing hash table built at
+// compile time from the same list.
+enum Dict : uint8_t { D_SPARSE, D_ANNOTATED };
+constexpr int kHashN = 1024;
+__host__ __device__ constexpr unsigned key_hash(const char *s, int n) {
+	unsigned h = 2166136261u; // FNV-1a
+	for (int i = 0; i < n; i++) h = (h ^ (unsigned char)s[i]) * 16777619u;
+	return h;
+}
+struct KeyHash {
+	int16_t k[kHashN];
+};
+constexpr KeyHash make_key_hash() {
+	KeyHash t{};
+	const char s[] = {
+#define X(n) #n "\0"
+		AJ_KEYS(X)
+#undef X
+	};
+	for (int i = 0; i < kHashN; i++) t.k[i] = -1;
+	for (int k = 0; k < K_COUNT; k++) {
+		const char *name = s + kKeyOff.o[k];
+		int n = 0;
+		while (name[n]) n++;
+		unsigned h = key_hash(name, n) % kHashN;
+		while (t.k[h] >= 0) h = (h + 1) % kHashN;
+		t.k[h] = (int16_t)k;
+	}
+	return t;
+}
+AJ_TABLE(KeyHash, key_hash_tab, 1, { make_key_hash() })
+
+// the key named s[0, n), or -1
+__host__ __device__ int find_key(const char *s, int n) {
+	const char *blob = AJ_TAB(key_blob)[0].s;
+	for (unsigned h = key_hash(s, n) % kHashN;; h = (h + 1) % kHashN) {
+		const int k = AJ_TAB(key_hash_tab)[0].k[h];
+		if (k < 0) return -1;
+		const char *name = blob + AJ_TAB(key_off)[0].o[k];
+		int i = 0;
+		while (i < n && name[i] == s[i]) i++;
+		if (i == n && !name[n]) return k;
+	}
+}
+
+// The full line in[0, n) (a flat object: numbers, strings, booleans, null and one array of strings) written in dictionary d, as
+// JSON::Serializer writes the same members: sparse -- each key renamed, a key without a sparse name left out with its value;
+// annotated -- each value as {"value":v[,"unit":..][,"description":..][,"text":..]}, "text" being the key's lookup entry for a
+// number's integer part (a number's value: the lookup keys hold integers).
+__host__ __device__ void rewrite(Out &o, const char *in, int n, int d) {
+	const char *blob = AF_TAB(af_blob)[0].s;
+	o.ch('{');
+	bool first = true;
+	int i = 1;
+	while (i < n && in[i] != '}') {
+		if (in[i] == ',') i++;
+		const int ks = i + 1;
+		int ke = ks;
+		while (ke < n && in[ke] != '"') ke++;
+		const int vs = ke + 2; // past '":'
+		int ve = vs, depth = 0;
+		bool str = false;
+		for (; ve < n; ve++) {
+			const char c = in[ve];
+			if (str) {
+				if (c == '\\') ve++;
+				else if (c == '"') str = false;
+			}
+			else if (c == '"') str = true;
+			else if (c == '[') depth++;
+			else if (c == ']') depth--;
+			else if ((c == ',' || c == '}') && depth == 0) break;
+		}
+		i = ve;
+		const int k = find_key(in + ks, ke - ks);
+		if (d == D_SPARSE) {
+			const char *name = k >= 0 ? blob + AF_TAB(af_sparse)[k] : "";
+			if (!*name) continue;
+			if (!first) o.ch(',');
+			o.ch('"');
+			o.cstr(name);
+			o.raw("\":", 2);
+			o.raw(in + vs, ve - vs);
+		}
+		else {
+			if (!first) o.ch(',');
+			o.raw(in + ks - 1, ke - ks + 3); // "key":
+			o.raw("{\"value\":", 9);
+			o.raw(in + vs, ve - vs);
+			if (k >= 0) {
+				const uint32_t u = AF_TAB(af_unit)[k], ds = AF_TAB(af_desc)[k];
+				if (u != 0xFFFFFFFFu) {
+					o.raw(",\"unit\":\"", 9);
+					o.cstr(blob + u);
+					o.ch('"');
+				}
+				if (ds != 0xFFFFFFFFu) {
+					o.raw(",\"description\":\"", 16);
+					o.cstr(blob + ds);
+					o.ch('"');
+				}
+				const int t = AF_TAB(af_lut)[k];
+				const char c0 = in[vs];
+				if (t >= 0 && ((c0 >= '0' && c0 <= '9') || c0 == '-')) {
+					long long v = 0;
+					for (int j = c0 == '-' ? vs + 1 : vs; j < ve && in[j] >= '0' && in[j] <= '9' && v < 1000000; j++) v = v * 10 + (in[j] - '0');
+					if (c0 == '-') v = -v;
+					if (v >= 0 && v < AF_TAB(af_lut_n)[t]) {
+						o.raw(",\"text\":\"", 9);
+						o.cstr(blob + AF_TAB(af_lut_text)[AF_TAB(af_lut_at)[t] + (int)v]);
+						o.ch('"');
+					}
+				}
+			}
+			o.ch('}');
+		}
+		first = false;
+	}
+	o.ch('}');
+}
+
+// seconds from microseconds the way getNMEAJSON prints rxuxtime / toa: integer when whole (Message.cpp:121-137)
+__host__ __device__ void usec(Out &o, long long t) {
+	if (t % 1000000 != 0) o.f64((double)t / 1000000.0);
+	else o.i64(t / 1000000);
+}
+
+// AIS::Message::getNMEAJSON (Message.cpp:93-191)
+__host__ __device__ void nmea_json(Out &o, const aisgpu_msg *m, const FmtCtx &c) {
+	o.cstr("{\"class\":\"AIS\",\"device\":\"AIS-catcher\",\"version\":");
+	o.i64(c.version);
+	o.cstr(",\"driver\":");
+	o.i64(c.driver);
+	o.cstr(",\"hardware\":");
+	o.qstr(c.hardware);
+	o.cstr(",\"channel\":\"");
+	o.ch(m->channel);
+	o.cstr("\",\"repeat\":");
+	o.i64(m->data[0] & 3); // Message::repeat(), Message.h:186-189
+	if (c.include_ssl) {
+		o.cstr(",\"ssc\":");
+		o.i64(m->start_idx);
+		o.cstr(",\"sl\":");
+		o.i64(m->end_idx - m->start_idx);
+	}
+	if (c.status) {
+		o.cstr(",\"msg_status\":");
+		o.i64(c.status);
+	}
+	if (c.mode & 2) {
+		o.cstr(",\"rxuxtime\":");
+		usec(o, c.rxtime_us);
+	}
+	if (c.toa_us != 0) {
+		o.cstr(",\"toa\":");
+		usec(o, c.toa_us);
+	}
+	if (c.uuid[0]) {
+		o.cstr(",\"uuid\":\"");
+		o.cstr(c.uuid); // copied verbatim, as the reference does
+		o.ch('"');
+	}
+	if (c.ipv4) {
+		o.cstr(",\"ipv4\":");
+		o.i64((long long)c.ipv4);
+	}
+	if (c.mode & 1) {
+		o.cstr(",\"signalpower\":");
+		if (m->level == 1024.0f) o.cstr("null"); // LEVEL_UNDEFINED
+		else o.f64((double)m->level);
+		o.cstr(",\"ppm\":");
+		if (m->ppm == 1024.0f) o.cstr("null"); // PPM_UNDEFINED
+		else o.f64((double)m->ppm);
+	}
+	if (c.station) {
+		o.cstr(",\"station_id\":");
+		o.i64(c.station);
+	}
+	if (m->nbits > 0) {
+		const unsigned mmsi = ((unsigned)m->data[1] << 22) | ((unsigned)m->data[2] << 14) | ((unsigned)m->data[3] << 6) | ((unsigned)m->data[4] >> 2);
+		o.cstr(",\"mmsi\":");
+		o.i64((long long)mmsi); // Message.h:191-194
+		o.cstr(",\"type\":");
+		o.i64(m->data[0] >> 2);
+	}
+	o.cstr(",\"nmea\":[");
+	for (int i = 0; i < n_sent(m); i++) {
+		if (i) o.ch(',');
+		o.ch('"');
+		o.raw(m->nmea[i], sent_len(m, i));
+		o.ch('"');
+	}
+	o.cstr("]}");
+	o.cstr(c.suffix);
+}
+
+// AIS::Message::getBinaryNMEA (Message.cpp:287-396): 0xAC 0x00 <flags> | the rest byte-stuffed: '\n' -> AD AE, '\r' -> AD AF,
+// 0xAD -> AD AD | '\n'; nothing for a length outside [0, 1064].  start: where the record began (the CRC covers it).
+__host__ __device__ void binary(Out &o, const char *start, const aisgpu_msg *m, long long rxtime_us, bool crc) {
+	if (m->nbits < 0 || m->nbits > kMaxBits) return;
+	const int nbytes = (m->nbits + 7) / 8;
+	auto put = [&](unsigned b) {
+		b &= 0xffu;
+		if (b == '\n' || b == '\r' || b == 0xad) {
+			o.ch((char)0xad);
+			o.ch((char)(b == '\n' ? 0xae : b == '\r' ? 0xaf : 0xad));
+		}
+		else o.ch((char)b);
+	};
+	o.ch((char)0xac);
+	o.ch((char)0x00);
+	unsigned flags = 0;
+	if (m->level != 1024.0f && m->ppm != 1024.0f) flags |= 1u;
+	if (crc) flags |= 2u;
+	o.ch((char)flags);
+	for (int i = 0; i < 8; i++) put((unsigned)((unsigned long long)rxtime_us >> ((7 - i) * 8))); // big-endian time stamp
+	if (flags & 1u) {
+		const int level10 = (int)(m->level * 10.0f);
+		put((unsigned)(level10 >> 8));
+		put((unsigned)level10);
+		const int ppm10 = (int)(m->ppm * 10.0f);
+		put((unsigned)(int8_t)ppm10);
+	}
+	o.ch(m->channel); // these two are written unescaped by the reference (Message.cpp:376-377)
+	o.ch((char)((m->nbits >> 8) & 0xff));
+	put((unsigned)m->nbits);
+	for (int i = 0; i < nbytes; i++) put(m->data[i]);
+	if (crc && !o.full) { // CRC-16/ARC style (reflected 0xA001, init 0xFFFF) over everything written so far, escapes included
+		unsigned cr = 0xffffu;
+		for (const unsigned char *q = (const unsigned char *)start; q < (const unsigned char *)o.p; q++) {
+			cr ^= *q;
+			for (int j = 0; j < 8; j++) cr = (cr & 1u) ? (cr >> 1) ^ 0xa001u : cr >> 1;
+		}
+		put(cr >> 8);
+		put(cr);
+	}
+	o.ch('\n');
+}
+
+// AIS::Message::getNMEATagBlock (Message.cpp:198-285) with the engine's group counter: groups = the multi-sentence frames before
+// this one
+__host__ __device__ void tag_block(Out &o, const aisgpu_msg *m, const FmtCtx &c, long long groups) {
+	const int total = n_sent(m);
+	const int group = total > 1 ? (int)(groups % 9999) + 1 : 0;
+	for (int seq = 1; seq <= total; seq++) {
+		char tb[96];
+		Out t(tb, (int)sizeof(tb));
+		t.raw("s:s", 3);
+		t.i64(c.station);
+		t.raw(",c:", 3);
+		t.f64((double)c.rxtime_us / 1000000.0);
+		if (total > 1) {
+			t.raw(",g:", 3);
+			t.i64(seq);
+			t.ch('-');
+			t.i64(total);
+			t.ch('-');
+			t.i64(group);
+		}
+		const int n = (int)(t.p - tb);
+		unsigned x = 0;
+		for (int i = 0; i < n; i++) x ^= (unsigned char)tb[i];
+		o.ch('\\');
+		o.raw(tb, n);
+		o.ch('*');
+		o.ch("0123456789ABCDEF"[(x >> 4) & 15]);
+		o.ch("0123456789ABCDEF"[x & 15]);
+		o.ch('\\');
+		o.raw(m->nmea[seq - 1], sent_len(m, seq - 1));
+		o.raw("\r\n", 2);
+	}
+}
+
+// the screen's annotated sentences (OutputMessage::formatInto, MsgOut.h:73-106)
+__host__ __device__ void full_text(Out &o, const aisgpu_msg *m, const FmtCtx &c) {
+	for (int i = 0; i < n_sent(m); i++) {
+		o.raw(m->nmea[i], sent_len(m, i));
+		o.raw(" ( ", 3);
+		if (m->nbits > 0) {
+			o.cstr("MSG: ");
+			o.u64(m->data[0] >> 2);
+			o.cstr(", REPEAT: ");
+			o.u64(m->data[0] & 3);
+			o.cstr(", MMSI: ");
+			o.u64(((unsigned)m->data[1] << 22) | ((unsigned)m->data[2] << 14) | ((unsigned)m->data[3] << 6) | ((unsigned)m->data[4] >> 2));
+		}
+		else o.cstr("empty");
+		if ((c.mode & 1) && m->ppm != 1024.0f && m->level != 1024.0f) {
+			o.cstr(", signalpower: ");
+			put_g(o, m->level);
+			o.cstr(", ppm: ");
+			put_g(o, m->ppm);
+		}
+		if (c.mode & 2) {
+			o.cstr(", timestamp: ");
+			put_rxtime(o, c.rxtime_us);
+		}
+		if (c.station) {
+			o.cstr(", ID: ");
+			o.i64(c.station);
+		}
+		o.raw(")\n", 2);
+	}
+}
+
+// one full-JSON line: prefix, body, '}'; its length, or -2 when it does not fit in cap
 __host__ __device__ int line(const aisgpu_msg *src, const char *prefix, int prefix_len, int mode, int station, char *out, int cap) {
 	Msg m;
 	for (int i = 0; i < kBufBytes; i++) m.d[i] = i < kMaxBytes ? src->data[i] : 0;
@@ -1178,31 +1645,94 @@ __host__ __device__ int line(const aisgpu_msg *src, const char *prefix, int pref
 	return o.full ? -2 : (int)(o.p - out);
 }
 
-__global__ void k_json_lines(const aisgpu_msg *__restrict__ msgs, int n, const char *__restrict__ prefix, int prefix_len, int mode,
-							 int station, char *__restrict__ slots, int slot, int *__restrict__ len) {
-	const int i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	len[i] = line(msgs + i, prefix, prefix_len, mode, station, slots + (size_t)i * slot, slot);
+// The record of one frame in c.fmt (OutputMessage::formatInto, MsgOut.h:58-122, and OutputMessage::Receive for the JSON formats):
+// its length, or -2 when it does not fit in cap.  ordinal: the frames published before it; groups: the multi-sentence ones among
+// them.  JSON_SPARSE and JSON_ANNOTATED write the full line into scratch (scap bytes) first and rewrite it into out.
+__host__ __device__ int record(const aisgpu_msg *src, const FmtCtx &c, long long ordinal, long long groups, char *out, int cap,
+							   char *scratch, int scap) {
+	Out o(out, cap);
+	switch (c.fmt) {
+	case AISGPU_MSGFORMAT_NMEA:
+		for (int i = 0; i < n_sent(src); i++) {
+			o.raw(src->nmea[i], sent_len(src, i));
+			o.cstr(c.suffix);
+		}
+		break;
+	case AISGPU_MSGFORMAT_NMEA_TAG: tag_block(o, src, c, groups); break;
+	case AISGPU_MSGFORMAT_COMMUNITY_HUB:
+		if (ordinal % 100 == 0) nmea_json(o, src, c);
+		else binary(o, out, src, c.rxtime_us, false);
+		break;
+	case AISGPU_MSGFORMAT_BINARY_NMEA: binary(o, out, src, c.rxtime_us, c.crc != 0); break;
+	case AISGPU_MSGFORMAT_FULL: full_text(o, src, c); break;
+	case AISGPU_MSGFORMAT_JSON_NMEA: nmea_json(o, src, c); break;
+	case AISGPU_MSGFORMAT_JSON_FULL: {
+		const int n = line(src, c.prefix, c.prefix_len, c.mode, c.station, out, cap);
+		if (n < 0) return -2;
+		o.p += n;
+		o.cstr(c.suffix);
+		break;
+	}
+	default: {
+		const int n = line(src, c.prefix, c.prefix_len, c.mode, c.station, scratch, scap);
+		if (n < 0) return -2;
+		rewrite(o, scratch, n, c.fmt == AISGPU_MSGFORMAT_JSON_SPARSE ? D_SPARSE : D_ANNOTATED);
+		o.cstr(c.suffix);
+		break;
+	}
+	}
+	return o.full ? -2 : (int)(o.p - out);
 }
 
-// Where each line goes: line i (its bytes and a newline) is kept when the lines of its submit up to and including it fit in cap
-// bytes, and kept lines are packed in frame order.  A submit that began in an earlier batch has already used carry bytes (lines
-// of the first submit of the batch count from -carry).  One block walks the batch in tiles of 256 frames twice: the running sum of
-// every line, then the running sum of the kept ones.
-__global__ void __launch_bounds__(256) k_json_place(const int *__restrict__ len, const int *__restrict__ seg, int n, long long cap,
-													long long carry, long long *__restrict__ psum, long long *__restrict__ off,
-													int *__restrict__ keep, long long *__restrict__ total) {
+// groups[i] = base + the multi-sentence frames of the batch before frame i; total[3] = those of the whole batch (one block, tiles of
+// 256 frames: an exclusive scan with a carried sum)
+__global__ void __launch_bounds__(256) k_fmt_groups(const aisgpu_msg *__restrict__ msgs, int n, long long base,
+													long long *__restrict__ groups, long long *__restrict__ total) {
 	typedef cub::BlockScan<long long, 256> Scan;
 	__shared__ typename Scan::TempStorage ts;
-	__shared__ long long s_carry, s_lines;
+	__shared__ long long s_carry;
+	if (threadIdx.x == 0) s_carry = base;
+	__syncthreads();
+	for (int t0 = 0; t0 < n; t0 += 256) {
+		const int i = t0 + threadIdx.x;
+		const long long f = i < n && msgs[i].n_sentences > 1 ? 1 : 0;
+		long long ex, agg;
+		Scan(ts).ExclusiveSum(f, ex, agg);
+		if (i < n) groups[i] = s_carry + ex;
+		__syncthreads();
+		if (threadIdx.x == 0) s_carry += agg;
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) total[3] = s_carry - base;
+}
+
+// record i (frame ordinal + i) into the first cap bytes of its slot, the rest of the slot its scratch; its length into len[i]
+__global__ void k_fmt_records(const aisgpu_msg *__restrict__ msgs, int n, const FmtCtx *__restrict__ ctx, long long ordinal,
+							  const long long *__restrict__ groups, char *__restrict__ slots, int slot, int cap, int *__restrict__ len) {
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	char *s = slots + (size_t)i * slot;
+	len[i] = record(msgs + i, *ctx, ordinal + i, groups[i], s, cap, s + cap, slot - cap);
+}
+
+// Where each record goes: record i is kept when the records of its submit up to and including it fit in cap bytes, and kept
+// records are packed in frame order.  A submit that began in an earlier batch has already used carry bytes (records of the first
+// submit of the batch count from -carry).  One block walks the batch in tiles of 256 frames twice: the running sum of every
+// record, then the running sum of the kept ones.  keep[i] = its bytes, -1 when it is dropped.
+__global__ void __launch_bounds__(256) k_fmt_place(const int *__restrict__ len, const int *__restrict__ seg, int n, long long cap,
+												   long long carry, long long *__restrict__ psum, long long *__restrict__ off,
+												   int *__restrict__ keep, long long *__restrict__ total) {
+	typedef cub::BlockScan<long long, 256> Scan;
+	__shared__ typename Scan::TempStorage ts;
+	__shared__ long long s_carry, s_kept;
 	if (threadIdx.x == 0) {
 		s_carry = 0;
-		s_lines = 0;
+		s_kept = 0;
 	}
 	__syncthreads();
 	for (int t0 = 0; t0 < n; t0 += 256) {
 		const int i = t0 + threadIdx.x;
-		const long long b = i < n ? (long long)(len[i] > 0 ? len[i] : 0) + 1 : 0; // a line too long for its slot (never: see json_slot) is ""
+		const long long b = i < n ? (long long)(len[i] > 0 ? len[i] : 0) : 0; // a record too long for its slot (never: see the slot) is ""
 		long long incl, agg;
 		Scan(ts).InclusiveSum(b, incl, agg);
 		if (i < n) psum[i] = s_carry + incl;
@@ -1215,43 +1745,51 @@ __global__ void __launch_bounds__(256) k_json_place(const int *__restrict__ len,
 	for (int t0 = 0; t0 < n; t0 += 256) {
 		const int i = t0 + threadIdx.x;
 		long long k = 0;
+		bool kept = false;
 		if (i < n) {
 			const long long before = seg[i] > 0 ? psum[seg[i] - 1] : -carry;
-			k = psum[i] - before <= cap ? psum[i] - (i > 0 ? psum[i - 1] : 0) : 0;
+			kept = psum[i] - before <= cap;
+			k = kept ? psum[i] - (i > 0 ? psum[i - 1] : 0) : 0;
 		}
 		long long ex, agg;
 		Scan(ts).ExclusiveSum(k, ex, agg);
 		if (i < n) {
-			keep[i] = (int)k;
+			keep[i] = kept ? (int)k : -1;
 			off[i] = s_carry + ex;
 		}
-		const int kept = __syncthreads_count(k > 0);
+		const int nk = __syncthreads_count(kept);
 		if (threadIdx.x == 0) {
 			s_carry += agg;
-			s_lines += kept;
+			s_kept += nk;
 		}
 		__syncthreads();
 	}
 	if (threadIdx.x == 0) {
 		total[0] = s_carry;
-		total[1] = s_lines;
+		total[1] = s_kept;
 		total[2] = psum[n - 1] - (seg[n - 1] > 0 ? psum[seg[n - 1] - 1] : -carry); // bytes of the last submit so far, for the next batch
 	}
 }
 
-// One warp per kept line: its bytes from the slot to the packed text, then the newline.
-__global__ void k_json_copy(const char *__restrict__ slots, int slot, const int *__restrict__ keep, const long long *__restrict__ off,
-							int n, char *__restrict__ text) {
+// One warp per kept record: its bytes from the slot to the packed text.
+__global__ void k_fmt_copy(const char *__restrict__ slots, int slot, const int *__restrict__ keep, const long long *__restrict__ off,
+						   int n, char *__restrict__ text) {
 	const int i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-	if (i >= n || !keep[i]) return;
-	const int l = keep[i] - 1;
+	if (i >= n || keep[i] <= 0) return;
+	const int l = keep[i];
 	const char *s = slots + (size_t)i * slot;
 	char *d = text + off[i];
 	for (int c = lane; c < l; c += 32) d[c] = s[c];
-	if (lane == 0) d[l] = '\n';
 }
 
 } // namespace
+
+int fmt_record_host(const aisgpu_msg *m, const FmtCtx *c, long long ordinal, long long groups, char *out, int cap) {
+	const bool rewritten = c->fmt == AISGPU_MSGFORMAT_JSON_SPARSE || c->fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED;
+	std::vector<char> scratch(rewritten ? (size_t)c->prefix_len + 4096 : 0);
+	const int n = record(m, *c, ordinal, groups, out, cap, scratch.data(), (int)scratch.size());
+	return n < 0 ? AISGPU_EOVERFLOW : n;
+}
 
 std::string aj_prefix(const aisgpu_tag *tag) {
 	std::string s(256 + (tag->hardware ? strlen(tag->hardware) * 6 : 0), '\0');
@@ -1263,21 +1801,8 @@ std::string aj_prefix(const aisgpu_tag *tag) {
 	o.cstr(",\"hardware\":");
 	o.qstr(tag->hardware ? tag->hardware : "");
 	if (tag->mode & 2) {
-		// Message::getRxTime: YYYYMMDDHHMMSS (UTC) of the whole seconds, times before the epoch as the epoch (days -> civil date)
-		long long t = tag->rxtime_us / 1000000;
-		if (t < 0) t = 0;
-		const int sec = (int)(t % 60), mn = (int)(t / 60 % 60), hr = (int)(t / 3600 % 24);
-		const int z = (int)(t / 86400) + 719468, era = (z >= 0 ? z : z - 146096) / 146097;
-		const unsigned doe = (unsigned)(z - era * 146097), yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
-		const unsigned doy = doe - (365 * yoe + yoe / 4 - yoe / 100), mp = (5 * doy + 2) / 153;
-		const int day = (int)(doy - (153 * mp + 2) / 5 + 1), mon = (int)(mp + (mp < 10 ? 3 : -9));
-		const int year = (int)yoe + era * 400 + (mon <= 2);
 		o.cstr(",\"rxtime\":\"");
-		const int parts[7] = { year / 100, year % 100, mon, day, hr, mn, sec };
-		for (int v : parts) {
-			o.ch((char)('0' + v / 10));
-			o.ch((char)('0' + v % 10));
-		}
+		put_rxtime(o, tag->rxtime_us); // Message::getRxTime
 		o.cstr("\",\"rxuxtime\":");
 		o.f64((double)tag->rxtime_us / 1000000.0);
 	}
@@ -1290,31 +1815,55 @@ std::string aj_prefix(const aisgpu_tag *tag) {
 	return s;
 }
 
-int aj_line_host(const aisgpu_msg *m, const char *prefix, int prefix_len, int mode, int station, char *out, int cap) {
-	const int n = line(m, prefix, prefix_len, mode, station, out, cap);
-	return n < 0 ? AISGPU_EOVERFLOW : n;
+cudaError_t fmt_launch(const aisgpu_msg *d_msgs, int n, const FmtCtx *d_ctx, long long ordinal, long long groups, long long *d_groups,
+					   char *d_slots, int slot, int cap, int *d_len, const int *d_seg, long long budget, long long carry,
+					   long long *d_psum, long long *d_off, int *d_keep, long long *d_total, char *d_text, cudaStream_t st) {
+	if (n <= 0) return cudaSuccess;
+	k_fmt_groups<<<1, 256, 0, st>>>(d_msgs, n, groups, d_groups, d_total);
+	k_fmt_records<<<(n + 127) / 128, 128, 0, st>>>(d_msgs, n, d_ctx, ordinal, d_groups, d_slots, slot, cap, d_len);
+	k_fmt_place<<<1, 256, 0, st>>>(d_len, d_seg, n, budget, carry, d_psum, d_off, d_keep, d_total);
+	k_fmt_copy<<<(n + 7) / 8, 256, 0, st>>>(d_slots, slot, d_keep, d_off, n, d_text);
+	return cudaGetLastError();
 }
 
-cudaError_t aj_launch(const aisgpu_msg *d_msgs, int n, const char *d_prefix, int prefix_len, int mode, int station, char *d_slots,
-					  int slot, int *d_len, const int *d_seg, long long cap, long long carry, long long *d_psum, long long *d_off, int *d_keep,
-					  long long *d_total, char *d_text, cudaStream_t st) {
-	if (n <= 0) return cudaSuccess;
-	k_json_lines<<<(n + 127) / 128, 128, 0, st>>>(d_msgs, n, d_prefix, prefix_len, mode, station, d_slots, slot, d_len);
-	k_json_place<<<1, 256, 0, st>>>(d_len, d_seg, n, cap, carry, d_psum, d_off, d_keep, d_total);
-	k_json_copy<<<(n + 7) / 8, 256, 0, st>>>(d_slots, slot, d_keep, d_off, n, d_text);
-	return cudaGetLastError();
+// the context of a tag: NULL strings as "" (suffix as given: NULL is none); prefix: aj_prefix(tag), which must outlive the context
+FmtCtx fmt_ctx(const aisgpu_tag *tag, int fmt, const char *suffix, const std::string &prefix) {
+	FmtCtx c;
+	c.fmt = fmt;
+	c.version = tag->version;
+	c.driver = tag->driver;
+	c.mode = tag->mode;
+	c.station = tag->station;
+	c.status = tag->status;
+	c.include_ssl = tag->include_ssl;
+	c.crc = 0;
+	c.ipv4 = tag->ipv4;
+	c.rxtime_us = tag->rxtime_us;
+	c.toa_us = tag->toa_us;
+	c.hardware = tag->hardware ? tag->hardware : "";
+	c.uuid = tag->uuid ? tag->uuid : "";
+	c.suffix = suffix ? suffix : "";
+	c.prefix = prefix.data();
+	c.prefix_len = (int)prefix.size();
+	return c;
 }
 
 extern "C" int aisgpu_msg_json_full(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int cap) {
 	if (!m || !tag || !out || cap <= 0) return AISGPU_EINVAL;
 	const std::string p = aj_prefix(tag);
-	int n = aj_line_host(m, p.data(), (int)p.size(), tag->mode, tag->station, out, cap);
-	if (n < 0) return n;
-	if (tag->suffix) {
-		const int k = (int)strlen(tag->suffix);
-		if (n + k > cap) return AISGPU_EOVERFLOW;
-		memcpy(out + n, tag->suffix, (size_t)k);
-		n += k;
+	const FmtCtx c = fmt_ctx(tag, AISGPU_MSGFORMAT_JSON_FULL, tag->suffix, p);
+	return fmt_record_host(m, &c, 0, 0, out, cap);
+}
+
+extern "C" int aisgpu_msg_format(const aisgpu_msg *m, const aisgpu_tag *tag, int msgformat, aisgpu_format_state *st, char *out, int cap) {
+	if (!m || !tag || !out || cap <= 0 || msgformat < AISGPU_MSGFORMAT_NMEA || msgformat > AISGPU_MSGFORMAT_JSON_ANNOTATED)
+		return AISGPU_EINVAL;
+	const std::string p = aj_prefix(tag);
+	const FmtCtx c = fmt_ctx(tag, msgformat, tag->suffix ? tag->suffix : "\r\n", p);
+	const int n = fmt_record_host(m, &c, st ? st->records : 0, st ? st->groups : 0, out, cap);
+	if (n >= 0 && st) {
+		st->records++;
+		if (m->n_sentences > 1) st->groups++;
 	}
 	return n;
 }

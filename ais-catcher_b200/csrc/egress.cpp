@@ -1,5 +1,6 @@
 // Egress formats for decoded frames (SURVEY.md 8f rank 4): what the reference's outputs make of an AIS::Message after the
-// demodulation path has produced it.  Host-only, no CUDA: these are pure formatters over aisgpu_msg.
+// demodulation path has produced it.  Host-only entry points over the host build of the record formatter in be_json.cu, the
+// code the engine runs on the device for aisgpu_poll_lines:
 //
 //   aisgpu_msg_json   == AIS::Message::getNMEAJSON   (Source/Marine/Message.cpp:93-191; number and string formatting of
 //                        JSON::Writer, Source/JSON/Writer.h:124-218, 269-345, 427-442)
@@ -10,221 +11,21 @@
 // in out).  The reference appends to a std::string; here the caller provides the buffer.
 
 #include "../../include/aisgpu.h"
+#include "be_json.h"
 
 #include <stdint.h>
-#include <string.h>
-
-namespace {
-
-const float kLevelUndefined = 1024.0f, kPpmUndefined = 1024.0f; // Source/Library/Common.h:214-215
-const int kMaxAisBits = 1064;                                    // MAX_AIS_LENGTH (Message.h:38)
-
-// bounded output cursor: writes are dropped once the buffer is full and the overflow is remembered
-struct Out {
-	char *p, *end;
-	bool full;
-	Out(char *b, int cap) : p(b), end(b + cap), full(false) {}
-	void ch(char c) {
-		if (p < end) *p++ = c;
-		else full = true;
-	}
-	void raw(const char *s, size_t n) {
-		for (size_t i = 0; i < n; i++) ch(s[i]);
-	}
-	void lit(const char *s) { raw(s, strlen(s)); }
-	void u64(unsigned long long v) {
-		char tmp[20];
-		int n = 0;
-		do {
-			tmp[n++] = (char)('0' + (int)(v % 10));
-			v /= 10;
-		} while (v);
-		while (n) ch(tmp[--n]);
-	}
-	void i64(long long v) {
-		if (v < 0) {
-			ch('-');
-			u64(0ULL - (unsigned long long)v);
-		}
-		else u64((unsigned long long)v);
-	}
-	// JSON::Writer::append_float: "null" outside (-1e18, 1e18) incl. NaN; otherwise whole part, then at most six decimals,
-	// rounded half-to-even on the sixth, trailing zeros trimmed, no point for integers (Writer.h:174-218, 427-442)
-	void f64(double v) {
-		if (!(v > -1e18 && v < 1e18)) {
-			lit("null");
-			return;
-		}
-		if (v < 0) {
-			ch('-');
-			v = -v;
-		}
-		long long whole = (long long)v;
-		const double scaled = (v - (double)whole) * 1000000.0;
-		int frac = (int)(scaled + 0.5);
-		if ((double)frac - scaled == 0.5 && (frac & 1)) frac--;
-		if (frac >= 1000000) {
-			whole++;
-			frac -= 1000000;
-		}
-		u64((unsigned long long)whole);
-		if (frac == 0) return;
-		char d[6];
-		for (int i = 5; i >= 0; i--) {
-			d[i] = (char)('0' + frac % 10);
-			frac /= 10;
-		}
-		int n = 6;
-		while (d[n - 1] == '0') n--;
-		ch('.');
-		raw(d, (size_t)n);
-	}
-	// JSON string with quotes; ", \ and control characters escaped (Writer.h:269-345)
-	void str(const char *s) {
-		ch('"');
-		for (; s && *s; s++) {
-			const unsigned char c = (unsigned char)*s;
-			switch (c) {
-			case '"': lit("\\\""); break;
-			case '\\': lit("\\\\"); break;
-			case '\b': lit("\\b"); break;
-			case '\f': lit("\\f"); break;
-			case '\n': lit("\\n"); break;
-			case '\r': lit("\\r"); break;
-			case '\t': lit("\\t"); break;
-			default:
-				if (c < 0x20) {
-					static const char hex[] = "0123456789abcdef";
-					lit("\\u00");
-					ch(hex[c >> 4]);
-					ch(hex[c & 15]);
-				}
-				else ch((char)c);
-			}
-		}
-		ch('"');
-	}
-	// seconds from microseconds the way the reference prints rxtime / toa: integer when whole (Message.cpp:121-137)
-	void usec(long long t) {
-		if (t % 1000000 != 0) f64((double)t / 1000000.0);
-		else i64(t / 1000000);
-	}
-};
-
-} // namespace
 
 extern "C" int aisgpu_msg_json(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int cap) {
 	if (!m || !tag || !out || cap <= 0 || m->n_sentences < 0 || m->n_sentences > 4) return AISGPU_EINVAL;
-	Out w(out, cap);
-	w.lit("{\"class\":\"AIS\",\"device\":\"AIS-catcher\",\"version\":");
-	w.i64(tag->version);
-	w.lit(",\"driver\":");
-	w.i64(tag->driver);
-	w.lit(",\"hardware\":");
-	w.str(tag->hardware ? tag->hardware : "");
-	w.lit(",\"channel\":\"");
-	w.ch(m->channel);
-	w.lit("\",\"repeat\":");
-	w.i64(m->data[0] & 3); // Message::repeat(), Message.h:186-189
-	if (tag->include_ssl) {
-		w.lit(",\"ssc\":");
-		w.i64(m->start_idx);
-		w.lit(",\"sl\":");
-		w.i64(m->end_idx - m->start_idx);
-	}
-	if (tag->status) {
-		w.lit(",\"msg_status\":");
-		w.i64(tag->status);
-	}
-	if (tag->mode & 2) {
-		w.lit(",\"rxuxtime\":");
-		w.usec(tag->rxtime_us);
-	}
-	if (tag->toa_us != 0) {
-		w.lit(",\"toa\":");
-		w.usec(tag->toa_us);
-	}
-	if (tag->uuid && tag->uuid[0]) {
-		w.lit(",\"uuid\":\"");
-		w.lit(tag->uuid); // copied verbatim, as the reference does
-		w.ch('"');
-	}
-	if (tag->ipv4) {
-		w.lit(",\"ipv4\":");
-		w.i64((long long)tag->ipv4);
-	}
-	if (tag->mode & 1) {
-		w.lit(",\"signalpower\":");
-		if (m->level == kLevelUndefined) w.lit("null");
-		else w.f64((double)m->level);
-		w.lit(",\"ppm\":");
-		if (m->ppm == kPpmUndefined) w.lit("null");
-		else w.f64((double)m->ppm);
-	}
-	if (tag->station) {
-		w.lit(",\"station_id\":");
-		w.i64(tag->station);
-	}
-	if (m->nbits > 0) {
-		const unsigned mmsi = ((unsigned)m->data[1] << 22) | ((unsigned)m->data[2] << 14) | ((unsigned)m->data[3] << 6) | ((unsigned)m->data[4] >> 2);
-		w.lit(",\"mmsi\":");
-		w.i64((long long)mmsi); // Message.h:191-194
-		w.lit(",\"type\":");
-		w.i64(m->data[0] >> 2);
-	}
-	w.lit(",\"nmea\":[");
-	for (int i = 0; i < m->n_sentences; i++) {
-		if (i) w.ch(',');
-		w.ch('"');
-		w.raw(m->nmea[i], (size_t)m->nmea_len[i]);
-		w.ch('"');
-	}
-	w.lit("]}");
-	if (tag->suffix) w.lit(tag->suffix);
-	return w.full ? AISGPU_EOVERFLOW : (int)(w.p - out);
+	const std::string no_prefix; // not printed by this format
+	const FmtCtx c = fmt_ctx(tag, AISGPU_MSGFORMAT_JSON_NMEA, tag->suffix, no_prefix);
+	return fmt_record_host(m, &c, 0, 0, out, cap);
 }
 
 extern "C" int aisgpu_msg_binary(const aisgpu_msg *m, const aisgpu_tag *tag, int crc, uint8_t *out, int cap) {
 	if (!m || !tag || !out || cap <= 0) return AISGPU_EINVAL;
-	if (m->nbits < 0 || m->nbits > kMaxAisBits) return 0; // the reference emits nothing for such a length (Message.cpp:279-280)
-	const int nbytes = (m->nbits + 7) / 8;
-	Out w((char *)out, cap);
-	// 0xAC 0x00 <flags> | the rest byte-stuffed: '\n' -> AD AE, '\r' -> AD AF, 0xAD -> AD AD | '\n'
-	auto put = [&](unsigned b) {
-		b &= 0xffu;
-		if (b == '\n' || b == '\r' || b == 0xad) {
-			w.ch((char)0xad);
-			w.ch((char)(b == '\n' ? 0xae : b == '\r' ? 0xaf : 0xad));
-		}
-		else w.ch((char)b);
-	};
-	w.ch((char)0xac);
-	w.ch((char)0x00);
-	unsigned flags = 0;
-	if (m->level != kLevelUndefined && m->ppm != kPpmUndefined) flags |= 1u;
-	if (crc) flags |= 2u;
-	w.ch((char)flags);
-	for (int i = 0; i < 8; i++) put((unsigned)((unsigned long long)tag->rxtime_us >> ((7 - i) * 8))); // big-endian time stamp
-	if (flags & 1u) {
-		const int level10 = (int)(m->level * 10.0f);
-		put((unsigned)(level10 >> 8));
-		put((unsigned)level10);
-		const int ppm10 = (int)(m->ppm * 10.0f);
-		put((unsigned)(int8_t)ppm10);
-	}
-	w.ch(m->channel);                   // these two are written unescaped by the reference (Message.cpp:376-377)
-	w.ch((char)((m->nbits >> 8) & 0xff));
-	put((unsigned)m->nbits);
-	for (int i = 0; i < nbytes; i++) put(m->data[i]);
-	if (crc && !w.full) { // CRC-16/ARC style (reflected 0xA001, init 0xFFFF) over everything written so far, escapes included
-		unsigned c = 0xffffu;
-		for (const unsigned char *q = out; q < (const unsigned char *)w.p; q++) {
-			c ^= *q;
-			for (int j = 0; j < 8; j++) c = (c & 1u) ? (c >> 1) ^ 0xa001u : c >> 1;
-		}
-		put(c >> 8);
-		put(c);
-	}
-	w.ch('\n');
-	return w.full ? AISGPU_EOVERFLOW : (int)(w.p - (char *)out);
+	const std::string no_prefix; // not printed by this format
+	FmtCtx c = fmt_ctx(tag, AISGPU_MSGFORMAT_BINARY_NMEA, nullptr, no_prefix);
+	c.crc = crc != 0;
+	return fmt_record_host(m, &c, 0, 0, (char *)out, cap);
 }

@@ -33,7 +33,8 @@ extern "C" {
 #endif
 
 /* 3 since the engine groups; later additions are new entry points only (the full AIS JSON: aisgpu_msg_json_full, aisgpu_json_enable,
- * aisgpu_poll_json), so the number callers check against stays 3.  A caller that needs those entry points looks them up
+ * aisgpu_poll_json; the output records: aisgpu_msg_format, aisgpu_lines_enable, aisgpu_poll_lines), so the number callers check
+ * against stays 3.  A caller that needs those entry points looks them up
  * (dlsym) instead of relying on the number. */
 #define AISGPU_ABI_VERSION 3
 
@@ -318,6 +319,74 @@ int aisgpu_msg_json_full(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, 
  * about 8.6 KB of device memory and 4.3 KB of pinned host memory per frame of a 4096-frame decode batch. */
 int aisgpu_json_enable(aisgpu_handle *h, const aisgpu_tag *tag, int max_bytes_per_submit);
 int aisgpu_poll_json(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_lines);
+
+/* Message formats: the position of each in the reference's enum class MessageFormat (Source/Library/Common.h:144-156), as MSGFORMAT
+ * selects them for an output (IO/MsgOut.h:282-289).  0 (SILENT) is not a format here.  The record of a frame is exactly what
+ * OutputMessage::formatInto (IO/MsgOut.h:58-122) -- or, for the three JSON formats, OutputMessage::Receive of the JSON stream --
+ * appends for that message, "suffix" being the output's line suffix (aisgpu_tag.suffix; NULL: "\r\n"):
+ *   NMEA           each sentence + suffix
+ *   NMEA_TAG       per sentence "\s:s<station>,c:<rxtime s>[,g:<i>-<n>-<group>]*hh\" + sentence + "\r\n" (getNMEATagBlock)
+ *   COMMUNITY_HUB  the JSON_NMEA record for the engine's frames 0, 100, 200, ...; the BINARY_NMEA record for the others
+ *   BINARY_NMEA    getBinaryNMEA(tag, crc = 0): possibly empty (aisgpu_msg_binary)
+ *   FULL           per sentence "<s> ( MSG: t, REPEAT: r, MMSI: m[, signalpower: %g, ppm: %g][, timestamp: YYYYMMDDHHMMSS][, ID: station])\n";
+ *                  signalpower / ppm when mode bit 0 is set and neither is 1024 (undefined), the timestamp when mode bit 1 is set
+ *   JSON_NMEA      getNMEAJSON(tag, include_ssl, uuid, suffix) (aisgpu_msg_json)
+ *   JSON_SPARSE    the full AIS JSON object under the sparse dictionary + suffix: keys renamed, a key without a sparse name left out
+ *                  with its value
+ *   JSON_FULL      the full AIS JSON line (aisgpu_msg_json_full) + suffix
+ *   JSON_ANNOTATED the full AIS JSON object with every member's value written as {"value":v[,"unit":..][,"description":..][,"text":..]}
+ *                  ("text": the lookup entry of a number's value, where its key has a table) + suffix
+ * JSON_SPARSE and JSON_ANNOTATED are the JSON_FULL line rewritten member by member, as JSON::Serializer writes the same members.
+ * Two counters make a record depend on the frames before it.  The reference keeps them per output (hub_lines) and per process (the
+ * NMEA_TAG group id); here both are the engine's, start at 0 as in a fresh process, and sit beside the per-stream NMEA sequence id
+ * (aisgpu_msg.nmea) as the engine's state:
+ *   - records: the frames the engine has published; COMMUNITY_HUB prints JSON_NMEA where it is a multiple of 100;
+ *   - groups: the multi-sentence frames among them; the k-th such frame has NMEA_TAG group ((k - 1) % 9999) + 1.
+ * Both advance over every published frame in emission order, including frames whose records the byte budget drops.  The engine
+ * computes them on the device (a scan with a base carried from one 4096-frame batch to the next); aisgpu_format_state is the same
+ * pair for aisgpu_msg_format. */
+#define AISGPU_MSGFORMAT_NMEA 1
+#define AISGPU_MSGFORMAT_NMEA_TAG 2
+#define AISGPU_MSGFORMAT_COMMUNITY_HUB 3
+#define AISGPU_MSGFORMAT_BINARY_NMEA 4
+#define AISGPU_MSGFORMAT_FULL 5
+#define AISGPU_MSGFORMAT_JSON_NMEA 6
+#define AISGPU_MSGFORMAT_JSON_SPARSE 7
+#define AISGPU_MSGFORMAT_JSON_FULL 8
+#define AISGPU_MSGFORMAT_JSON_ANNOTATED 9
+
+/* The engine's counters (above), for the host formatter. */
+typedef struct aisgpu_format_state {
+	int64_t records; /* frames formatted so far */
+	int64_t groups;  /* multi-sentence frames among them */
+} aisgpu_format_state;
+
+/* The record of m in msgformat (1..9), printed with *tag (version, driver, hardware, mode, status, ipv4, rxtime_us, toa_us, station,
+ * include_ssl, uuid; suffix NULL: "\r\n"), by the code the engine runs on the device for aisgpu_poll_lines, built for the host.
+ * With st (may be NULL: both counters 0), the record uses *st and, when it is written, advances it exactly as the engine advances
+ * its counters (records by one, groups by one for a frame of more than one sentence): a caller that formats every frame aisgpu_poll
+ * returns, in order, from a zeroed state gets the engine's records.  Sentence lengths (nmea_len) are taken up to the 100 bytes of
+ * aisgpu_msg.nmea, here and in aisgpu_msg_json.
+ * Returns the bytes written (no NUL; 0 for an empty record), AISGPU_EOVERFLOW if cap is too small (st unchanged), AISGPU_EINVAL
+ * for a NULL argument or an unknown format.  Host-only. */
+int aisgpu_msg_format(const aisgpu_msg *m, const aisgpu_tag *tag, int msgformat, aisgpu_format_state *st, char *out, int cap);
+
+/* The records of every published frame in one format, formatted on the GPU.  aisgpu_lines_enable (before the first submit; once,
+ * and not together with aisgpu_json_enable: one engine has one format) fixes the format, the tag every record is printed with (as
+ * for aisgpu_msg_format) and max_bytes_per_submit, the bytes one submit's records may take.  From then on every poll of the frame
+ * ring formats the frames it publishes on the device, exactly as aisgpu_json_enable decodes them (which is this with JSON_FULL and
+ * suffix "\n"): frames, taps and counters do not change, a group member formats its own frames, both queues are bounded by
+ * max_frames, and records past a submit's budget are dropped and reported as AISGPU_EOVERFLOW by the next aisgpu_poll_lines.
+ *
+ * aisgpu_poll_lines is aisgpu_poll_upto for the records: it copies whole records, in the order aisgpu_poll returns the frames, until
+ * the next would pass cap; *n_bytes and *n_records receive what was written.  Record i is frame i, also when it is empty (a
+ * BINARY_NMEA frame of no valid length).  AISGPU_EINVAL when no format is enabled, or when cap is smaller than the next record.
+ * aisgpu_poll_json reads the same queue on an engine enabled with aisgpu_json_enable, and is AISGPU_EINVAL on one enabled with
+ * aisgpu_lines_enable.  The engine allocates, at enable, a slot per frame of a 4096-frame batch on the device and pinned host room
+ * for the text: about 4.3 KB each (NMEA .. JSON_FULL), 8.5 / 4.3 KB (JSON_SPARSE) or 25 / 20.6 KB (JSON_ANNOTATED), plus the tag's
+ * strings. */
+int aisgpu_lines_enable(aisgpu_handle *h, int msgformat, const aisgpu_tag *tag, int max_bytes_per_submit);
+int aisgpu_poll_lines(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_records);
 
 /* == AIS::Message::getBinaryNMEA(out, tag, crc) (Message.cpp:277-396): 0xAC 0x00 framed, byte-stuffed binary record with an
  * optional CRC-16 (Helper.cpp:42-57).  Returns the bytes written, 0 when the reference would emit nothing. Host-only. */
