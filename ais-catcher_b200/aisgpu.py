@@ -26,7 +26,7 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
            "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files",
            "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json", "aisgpu_msg_format", "aisgpu_lines_enable",
-           "aisgpu_poll_lines"]
+           "aisgpu_poll_lines", "aisgpu_set_receivers", "aisgpu_check_receivers"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 # message formats: positions in the reference's enum class MessageFormat (MSGFORMAT of its outputs); include/aisgpu.h describes each record
@@ -61,6 +61,34 @@ class TagStruct(C.Structure):
     _fields_ = [("version", C.c_int32), ("driver", C.c_int32), ("hardware", C.c_char_p), ("mode", C.c_int32), ("status", C.c_int32),
                 ("ipv4", C.c_uint32), ("rxtime_us", C.c_int64), ("toa_us", C.c_int64), ("station", C.c_int32),
                 ("include_ssl", C.c_int32), ("uuid", C.c_char_p), ("suffix", C.c_char_p)]
+
+
+class Receiver(C.Structure):
+    """aisgpu_receiver: one stream's receiver (channel letters, station, own MMSI, tag mode, and the TAG's driver, hardware, ipv4)."""
+    _fields_ = [("channel_a", C.c_char), ("channel_b", C.c_char), ("station", C.c_int32), ("own_mmsi", C.c_int32),
+                ("tag_mode", C.c_uint32), ("driver", C.c_int32), ("hardware", C.c_char_p), ("ipv4", C.c_uint32)]
+
+
+def make_receiver(channels="AB", station=0, own_mmsi=-1, tag_mode=3, driver=0, hardware=None, ipv4=0):
+    """A Receiver from keyword arguments; channels: the two designation letters (X mode: the second is not read)."""
+    enc = lambda t: None if t is None else (t if isinstance(t, bytes) else t.encode("latin-1"))
+    ch = channels.encode("latin-1") if isinstance(channels, str) else bytes(channels)
+    return Receiver(ch[0:1], ch[1:2] or ch[0:1], station, own_mmsi, tag_mode, driver, enc(hardware), ipv4)
+
+
+def receiver_table(receivers):
+    """A ctypes array of Receiver from Receiver structures or dicts of make_receiver keyword arguments."""
+    rs = [r if isinstance(r, Receiver) else make_receiver(**r) for r in receivers]
+    return (Receiver * max(len(rs), 1))(*rs)
+
+
+def check_receivers(receivers, **engine):
+    """aisgpu_check_receivers (no GPU needed): the rules of Engine.set_receivers for an engine of keyword arguments `engine`.
+    Raises with the reason (the reference's text for a bad letter) if the table would be refused."""
+    lib = load()
+    rc = lib.aisgpu_check_receivers(C.byref(make_config(**engine)), receiver_table(receivers), len(receivers))
+    if rc:
+        raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode("latin-1")))
 
 
 MSG_FN = C.CFUNCTYPE(None, C.POINTER(MsgStruct), C.c_int, C.c_void_p)
@@ -146,6 +174,9 @@ def load():
                                           C.c_int]
         lib.aisgpu_lines_enable.argtypes = [C.c_void_p, C.c_int, C.POINTER(TagStruct), C.c_int]
         lib.aisgpu_poll_lines.argtypes = [C.c_void_p, C.c_int64, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_int)]
+    if hasattr(lib, "aisgpu_set_receivers"):  # absent from libraries built before the receiver tables (AISGPU_LIB)
+        lib.aisgpu_set_receivers.argtypes = [C.c_void_p, C.POINTER(Receiver), C.c_int]
+        lib.aisgpu_check_receivers.argtypes = [C.POINTER(Config), C.POINTER(Receiver), C.c_int]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -483,6 +514,13 @@ class Engine:
         records per submit."""
         self._json_tag = tag if tag is not None else make_tag()
         self._chk(self.lib.aisgpu_lines_enable(self.h, int(fmt), C.byref(self._json_tag), int(max_bytes_per_submit)))
+
+    def set_receivers(self, receivers):
+        """aisgpu_set_receivers: one receiver per stream (Receiver structures or dicts of make_receiver keyword arguments), before
+        the first submit and at most once.  Stream s then has receivers[s]'s letters, own MMSI and tag mode, and its records are
+        printed with its station, driver, hardware, mode and ipv4."""
+        self._receivers = receiver_table(receivers)  # copied by the library; kept anyway
+        self._chk(self.lib.aisgpu_set_receivers(self.h, self._receivers, len(receivers)))
 
     def poll_lines(self, ticket=None, cap=1 << 20):
         """aisgpu_poll_lines: (bytes, number of records) of the frames of the submits up to ticket (None: all), in frame order."""

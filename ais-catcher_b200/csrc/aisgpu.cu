@@ -105,6 +105,17 @@ enum Stage {
 	NSTAGE
 };
 
+// What aisgpu_set_receivers gives each stream: its channel letters, own MMSI and tag mode (what drain_ring reads), and the TAG fields
+// its records are printed with.  Without a table every stream holds the config's fields.
+struct Receiver {
+	char channel_a = 'A', channel_b = 'B';
+	int32_t station = 0, own_mmsi = -1;
+	uint32_t tag_mode = 3;
+	int32_t driver = 0;
+	std::string hardware;
+	uint32_t ipv4 = 0;
+};
+
 } // namespace
 
 struct aisgpu_handle {
@@ -218,6 +229,7 @@ struct aisgpu_handle {
 	int dwords = 0;
 	DecState *d_dec = nullptr;
 	uint32_t *d_dec_data = nullptr;
+	uint32_t *d_level_rows = nullptr; // bit per row: its frames carry the signal level (FrameOut::level_rows)
 	PllState *d_pll = nullptr;
 	V2State *d_v2 = nullptr;     // V2 engine: per-row state
 	float2 *d_Ed = nullptr;      // ModelChallenger: derotated 48 kHz samples [rows][HD + nE]
@@ -247,6 +259,8 @@ struct aisgpu_handle {
 	std::vector<aisgpu_msg> out_queue;
 	size_t out_pos = 0;
 	std::vector<int> seq; // per-stream multi-sentence sequence id (Message.cpp:28-39 is process-global in the reference)
+	std::vector<Receiver> rx; // per stream: the config's fields, or the receiver aisgpu_set_receivers installed
+	bool rx_table = false;    // aisgpu_set_receivers has been called: the records take the receivers' TAG fields
 	// last-submit geometry (for taps)
 	int last_n = 0, last_n48 = 0, last_nE = 0, last_nsym = 0, last_launches = 0;
 	uint64_t counters[8] = { 0 };
@@ -300,8 +314,12 @@ struct aisgpu_handle {
 	bool json_on = false, json_api = false;
 	int fmt = 0, json_slot = 0, rec_cap = 0;
 	long long json_cap = 0, fmt_records = 0, fmt_groups = 0;
-	std::string fmt_strings; // the tag's strings: hardware, uuid, suffix and the full-JSON prefix, each NUL-terminated
-	FmtCtx *d_fctx = nullptr;
+	// The output's tag (its strings owned here): with a receiver table, stream s's records are printed with it and s's receiver's
+	// station, driver, hardware, mode and ipv4, one context per stream.
+	aisgpu_tag fmt_tag = {};
+	std::string fmt_hw, fmt_uuid, fmt_suffix;
+	std::string fmt_strings; // uuid and suffix, then every context's hardware and full-JSON prefix, each NUL-terminated
+	FmtCtx *d_fctx = nullptr; // [1], or [n_streams] with a receiver table
 	cudaStream_t json_stream = nullptr;
 	char *d_jstrings = nullptr, *d_jslots = nullptr, *d_jtext = nullptr;
 	aisgpu_msg *d_jmsg = nullptr;
@@ -369,6 +387,22 @@ int halloc(aisgpu_handle *h, T **p, size_t n) { // pinned host memory
 	return 0;
 }
 
+// Releases a buffer of dalloc / halloc before the handle is destroyed (nothing may still use it)
+template <typename T>
+void dfree(aisgpu_handle *h, T *&p) {
+	if (!p) return;
+	h->dev_mem.erase(std::find(h->dev_mem.begin(), h->dev_mem.end(), (void *)p));
+	cudaFree(p);
+	p = nullptr;
+}
+template <typename T>
+void hfree(aisgpu_handle *h, T *&p) {
+	if (!p) return;
+	h->host_mem.erase(std::find(h->host_mem.begin(), h->host_mem.end(), (void *)p));
+	cudaFreeHost(p);
+	p = nullptr;
+}
+
 cudaError_t new_event(aisgpu_handle *h, cudaEvent_t *ev, unsigned flags = cudaEventDisableTiming) {
 	const cudaError_t e = cudaEventCreateWithFlags(ev, flags);
 	if (e == cudaSuccess) h->events.push_back(*ev);
@@ -379,7 +413,7 @@ cudaError_t new_event(aisgpu_handle *h, cudaEvent_t *ev, unsigned flags = cudaEv
 // when they were launched (mark_ticket keeps that limit for drain_ring).
 FrameOut frame_out(const aisgpu_handle *h) {
 	return FrameOut{ h->d_ring, h->d_ring_head, h->drained + (unsigned long long)h->ring_cap, h->ring_cap, (int)h->msg_chunk, (int)h->chunk,
-					 (h->cfg.tag_mode & 1) ? 1 : 0 };
+					 h->d_level_rows };
 }
 
 void set_frame_out(K3Params &p, const FrameOut &o) {
@@ -389,7 +423,18 @@ void set_frame_out(K3Params &p, const FrameOut &o) {
 	p.ring_cap = o.ring_cap;
 	p.chunk = o.chunk;
 	p.blk = o.blk;
-	p.mode_level = o.mode_level;
+	p.level_rows = o.level_rows;
+}
+
+// The level switch of every row from its stream's tag mode (bit 0: the frames carry the signal level, AIS.cpp:73-75) into
+// d_level_rows, before the first submit
+int put_level_rows(aisgpu_handle *h) {
+	std::vector<uint32_t> bits((size_t)(h->rows + 31) / 32, 0u);
+	for (int r = 0; r < h->rows; r++)
+		if (h->rx[stream_of_row(h, r)].tag_mode & 1) bits[r >> 5] |= 1u << (r & 31);
+	CU(cudaMemcpyAsync(h->d_level_rows, bits.data(), bits.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->stream));
+	CU(cudaStreamSynchronize(h->stream));
+	return 0;
 }
 
 bool has_cic(const aisgpu_handle *h) { return h->pre_us || h->kA > 0; }
@@ -1549,7 +1594,7 @@ int json_decode(aisgpu_handle *h, size_t q0) {
 		if (b0 == 0 || q[0].chunk != q[-1].chunk) carry = 0;
 		CU(cudaMemcpyAsync(h->d_jmsg, q, (size_t)n * sizeof(aisgpu_msg), cudaMemcpyHostToDevice, st));
 		CU(cudaMemcpyAsync(h->d_jseg, h->json_seg.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-		CU(fmt_launch(h->d_jmsg, n, h->d_fctx, h->fmt_records, h->fmt_groups, h->d_jgroups, h->d_jslots, h->json_slot, h->rec_cap,
+		CU(fmt_launch(h->d_jmsg, n, h->d_fctx, h->rx_table, h->fmt_records, h->fmt_groups, h->d_jgroups, h->d_jslots, h->json_slot, h->rec_cap,
 					  h->d_jlen, h->d_jseg, h->json_cap, carry, h->d_jpsum, h->d_joff, h->d_jkeep, h->d_jtotal, h->d_jtext, st));
 		CU(cudaMemcpyAsync(h->pin_jtotal, h->d_jtotal, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
 		CU(cudaMemcpyAsync(h->pin_jkeep, h->d_jkeep, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1652,18 +1697,19 @@ int drain_ring(aisgpu_handle *h, long long upto) {
 		aisgpu_msg m;
 		memset(&m, 0, sizeof(m));
 		m.stream = stream_of_row(h, r.row);
-		m.channel = channel_of_row(h, r.row) ? h->cfg.channel_b : h->cfg.channel_a;
+		const Receiver &rx = h->rx[m.stream]; // the config's fields unless a receiver table was installed
+		m.channel = channel_of_row(h, r.row) ? rx.channel_b : rx.channel_a;
 		m.nbits = (r.nbits >= 0 && r.nbits <= 1064) ? r.nbits : 0; // Message::setLength (Message.h:288-292)
 		m.start_idx = r.start_idx;
 		m.end_idx = r.end_idx;
 		m.ppm = r.ppm;
 		m.chunk = r.chunk;
 		float lvl = r.level;
-		if ((h->cfg.tag_mode & 1) && lvl != 0.0) lvl = (float)(10.0f * log10((double)lvl)); // AIS.cpp:74-75: the reference resolves to the double log10
+		if ((rx.tag_mode & 1) && lvl != 0.0) lvl = (float)(10.0f * log10((double)lvl)); // AIS.cpp:74-75: the reference resolves to the double log10
 		m.level = lvl;
 		memcpy(m.data, r.data, 140);
 		if (!msg_validate(m.data, m.nbits)) continue; // AIS.cpp:87-93: dropped, siblings were still reset
-		build_nmea(m, h->cfg.own_mmsi, &h->seq[m.stream]);
+		build_nmea(m, rx.own_mmsi, &h->seq[m.stream]);
 		h->counters[1]++;
 		h->counters[channel_of_row(h, r.row) ? 6 : 5]++;
 		h->out_queue.push_back(m);
@@ -1804,6 +1850,15 @@ static int create_impl(aisgpu_handle *h) {
 	h->inner_max = h->pre_dsk ? h->blk : (h->pre_us ? (maxN >> h->kA) : maxN);
 	h->max_n48 = h->inner_max >> ((h->xmode || h->disc) ? k : k + 1);
 	h->seq.assign(B, 0);
+	{
+		Receiver r;
+		r.channel_a = c.channel_a;
+		r.channel_b = c.channel_b;
+		r.station = c.station;
+		r.own_mmsi = c.own_mmsi;
+		r.tag_mode = c.tag_mode;
+		h->rx.assign(B, r);
+	}
 	// a group member (aisgpu_attach) has no front end: no pre-stage, warm-up tails, Rotate tables or input staging
 	if ((h->pre_us || h->pre_dsk) && !h->member) { // resampler pre-stage: raw-format history, level-kA stream, schedule tables, rings
 		const int tl = raw_tail_len(h);
@@ -1864,6 +1919,8 @@ static int create_impl(aisgpu_handle *h) {
 	const int ndec = h->chain == Chain::V2 ? 6 : (c.model == AISGPU_MODEL_CHALLENGER ? 10 : 5); // decoders per row
 	if (int rc = dalloc(h, &h->d_dec, (size_t)h->rows * ndec)) return rc;
 	if (int rc = dalloc(h, &h->d_dec_data, (size_t)h->rows * ndec * DEC_WORDS)) return rc;
+	if (int rc = dalloc(h, &h->d_level_rows, (size_t)(h->rows + 31) / 32)) return rc;
+	if (int rc = put_level_rows(h)) return rc;
 	if (int rc = h->chain == Chain::Fm ? alloc_fm(h, nEmax) : h->chain == Chain::Coherent ? alloc_coherent(h, nEmax) : alloc_v2(h)) return rc;
 	if (c.enable_taps)
 		if (int rc = dalloc(h, &h->d_tap_dec, (size_t)h->rows * 5 * (nEmax / 5 + 2))) return rc;
@@ -2083,6 +2140,92 @@ int aisgpu_poll(aisgpu_handle *h, aisgpu_msg *out, int max, int *n) { return ais
 
 namespace {
 
+// The tag stream s's records are printed with: the output's, with a receiver table the receiver's station, driver, hardware, mode
+// and ipv4
+aisgpu_tag tag_of(const aisgpu_handle *h, int s) {
+	aisgpu_tag t = h->fmt_tag;
+	t.hardware = h->fmt_hw.c_str();
+	t.uuid = h->fmt_uuid.c_str();
+	t.suffix = h->fmt_suffix.c_str();
+	if (h->rx_table) {
+		const Receiver &r = h->rx[s];
+		t.station = r.station;
+		t.driver = r.driver;
+		t.hardware = r.hardware.c_str();
+		t.mode = (int32_t)r.tag_mode;
+		t.ipv4 = r.ipv4;
+	}
+	return t;
+}
+
+// The format's contexts -- one, or one per stream with a receiver table -- with their strings in one packed buffer, and the slots and
+// text sized for the longest of them.  lines_enable calls it, and aisgpu_set_receivers again when a format is already enabled: the
+// buffers that depend on the strings are then made anew (nothing has been submitted, so nothing uses them).
+int fmt_setup(aisgpu_handle *h) {
+	const int nctx = h->rx_table ? h->cfg.n_streams : 1;
+	std::vector<aisgpu_tag> tags((size_t)nctx);
+	std::vector<std::string> prefixes((size_t)nctx);
+	std::vector<size_t> hw_at((size_t)nctx), prefix_at((size_t)nctx);
+	std::string strings = h->fmt_uuid + '\0' + h->fmt_suffix + '\0';
+	size_t longest = 0, longest_prefix = 0;
+	for (int i = 0; i < nctx; i++) {
+		tags[i] = tag_of(h, i);
+		prefixes[i] = aj_prefix(&tags[i]);
+		hw_at[i] = strings.size();
+		strings += std::string(tags[i].hardware) + '\0';
+		prefix_at[i] = strings.size();
+		strings += prefixes[i] + '\0';
+		longest = std::max(longest, prefixes[i].size() + strlen(tags[i].hardware) * 6);
+		longest_prefix = std::max(longest_prefix, prefixes[i].size());
+	}
+	h->fmt_strings = strings;
+	// a record's room: the longest record of its format with the tag's strings (the hardware name escaped, uuid and suffix once per
+	// sentence) -- four fully escaped sentences (2.4 KB) plus the longest fields (1.3 KB) after the full-JSON prefix, and for
+	// JSON_ANNOTATED their units and descriptions besides; JSON_SPARSE and JSON_ANNOTATED add a scratch full line to the slot
+	const size_t strs = longest + (h->fmt_uuid.size() + h->fmt_suffix.size()) * 4;
+	const int fmt = h->fmt;
+	const bool rewritten = fmt == AISGPU_MSGFORMAT_JSON_SPARSE || fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED;
+	h->rec_cap = (int)((strs + (fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED ? 20480 : 4096) + 15) / 16 * 16);
+	h->json_slot = h->rec_cap + (rewritten ? (int)((longest_prefix + 4096 + 15) / 16 * 16) : 0);
+	if (!h->json_stream) {
+		CU(cudaStreamCreateWithFlags(&h->json_stream, cudaStreamNonBlocking));
+		if (int rc = dalloc(h, &h->d_jtotal, 4)) return rc;
+		if (int rc = halloc(h, &h->pin_jtotal, 4)) return rc;
+		if (int rc = dalloc(h, &h->d_jmsg, kJsonBatch)) return rc;
+		if (int rc = dalloc(h, &h->d_jlen, kJsonBatch)) return rc;
+		if (int rc = dalloc(h, &h->d_jseg, kJsonBatch)) return rc;
+		if (int rc = dalloc(h, &h->d_jkeep, kJsonBatch)) return rc;
+		if (int rc = halloc(h, &h->pin_jkeep, kJsonBatch)) return rc;
+		if (int rc = dalloc(h, &h->d_jgroups, kJsonBatch)) return rc;
+		if (int rc = dalloc(h, &h->d_jpsum, kJsonBatch)) return rc;
+		if (int rc = dalloc(h, &h->d_joff, kJsonBatch)) return rc;
+	}
+	dfree(h, h->d_jstrings);
+	dfree(h, h->d_fctx);
+	dfree(h, h->d_jslots);
+	dfree(h, h->d_jtext);
+	hfree(h, h->pin_jtext);
+	const size_t text = (size_t)kJsonBatch * h->rec_cap;
+	if (int rc = dalloc(h, &h->d_jstrings, strings.size())) return rc;
+	if (int rc = dalloc(h, &h->d_fctx, (size_t)nctx)) return rc;
+	if (int rc = dalloc(h, &h->d_jslots, (size_t)kJsonBatch * h->json_slot)) return rc;
+	if (int rc = dalloc(h, &h->d_jtext, text)) return rc;
+	if (int rc = halloc(h, &h->pin_jtext, text)) return rc;
+	// dalloc zeroes each buffer on h->stream: the strings and the contexts are written after that, not under it
+	CU(cudaStreamSynchronize(h->stream));
+	CU(cudaMemcpy(h->d_jstrings, strings.data(), strings.size(), cudaMemcpyHostToDevice));
+	std::vector<FmtCtx> ctx((size_t)nctx);
+	for (int i = 0; i < nctx; i++) {
+		ctx[i] = fmt_ctx(&tags[i], fmt, h->fmt_suffix.c_str(), prefixes[i]);
+		ctx[i].uuid = h->d_jstrings;
+		ctx[i].suffix = h->d_jstrings + h->fmt_uuid.size() + 1;
+		ctx[i].hardware = h->d_jstrings + hw_at[i];
+		ctx[i].prefix = h->d_jstrings + prefix_at[i];
+	}
+	CU(cudaMemcpy(h->d_fctx, ctx.data(), ctx.size() * sizeof(FmtCtx), cudaMemcpyHostToDevice));
+	return 0;
+}
+
 // aisgpu_lines_enable and aisgpu_json_enable (who: the entry point, for the messages)
 int lines_enable(aisgpu_handle *h, int fmt, const aisgpu_tag *tag, const char *suffix, int max_bytes_per_submit, bool json_api,
 				 const char *who) {
@@ -2095,45 +2238,14 @@ int lines_enable(aisgpu_handle *h, int fmt, const aisgpu_tag *tag, const char *s
 		h->err = std::string(who) + (h->json_on ? ": a format is already enabled" : ": the engine has been submitted to");
 		return AISGPU_EINVAL;
 	}
-	const char *hw = tag->hardware ? tag->hardware : "", *uuid = tag->uuid ? tag->uuid : "";
-	const std::string prefix = aj_prefix(tag);
-	h->fmt_strings = std::string(hw) + '\0' + uuid + '\0' + suffix + '\0' + prefix + '\0';
+	h->fmt_tag = *tag;
+	h->fmt_hw = tag->hardware ? tag->hardware : "";
+	h->fmt_uuid = tag->uuid ? tag->uuid : "";
+	h->fmt_suffix = suffix;
 	h->fmt = fmt;
 	h->json_api = json_api;
 	h->json_cap = max_bytes_per_submit;
-	// a record's room: the longest record of its format with the tag's strings (the hardware name escaped, uuid and suffix once per
-	// sentence) -- four fully escaped sentences (2.4 KB) plus the longest fields (1.3 KB) after the full-JSON prefix, and for
-	// JSON_ANNOTATED their units and descriptions besides; JSON_SPARSE and JSON_ANNOTATED add a scratch full line to the slot
-	const size_t strs = prefix.size() + strlen(hw) * 6 + (strlen(uuid) + strlen(suffix)) * 4;
-	const bool rewritten = fmt == AISGPU_MSGFORMAT_JSON_SPARSE || fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED;
-	h->rec_cap = (int)((strs + (fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED ? 20480 : 4096) + 15) / 16 * 16);
-	h->json_slot = h->rec_cap + (rewritten ? (int)((prefix.size() + 4096 + 15) / 16 * 16) : 0);
-	CU(cudaStreamCreateWithFlags(&h->json_stream, cudaStreamNonBlocking));
-	const size_t text = (size_t)kJsonBatch * h->rec_cap;
-	if (int rc = dalloc(h, &h->d_jstrings, h->fmt_strings.size())) return rc;
-	if (int rc = dalloc(h, &h->d_fctx, 1)) return rc;
-	if (int rc = dalloc(h, &h->d_jtotal, 4)) return rc;
-	if (int rc = halloc(h, &h->pin_jtotal, 4)) return rc;
-	if (int rc = dalloc(h, &h->d_jmsg, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_jslots, (size_t)kJsonBatch * h->json_slot)) return rc;
-	if (int rc = dalloc(h, &h->d_jtext, text)) return rc;
-	if (int rc = halloc(h, &h->pin_jtext, text)) return rc;
-	if (int rc = dalloc(h, &h->d_jlen, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_jseg, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_jkeep, kJsonBatch)) return rc;
-	if (int rc = halloc(h, &h->pin_jkeep, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_jgroups, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_jpsum, kJsonBatch)) return rc;
-	if (int rc = dalloc(h, &h->d_joff, kJsonBatch)) return rc;
-	// dalloc zeroes each buffer on h->stream: the strings and the context are written after that, not under it
-	CU(cudaStreamSynchronize(h->stream));
-	CU(cudaMemcpy(h->d_jstrings, h->fmt_strings.data(), h->fmt_strings.size(), cudaMemcpyHostToDevice));
-	FmtCtx c = fmt_ctx(tag, fmt, suffix, prefix);
-	c.hardware = h->d_jstrings;
-	c.uuid = c.hardware + strlen(hw) + 1;
-	c.suffix = c.uuid + strlen(uuid) + 1;
-	c.prefix = c.suffix + strlen(suffix) + 1;
-	CU(cudaMemcpy(h->d_fctx, &c, sizeof(c), cudaMemcpyHostToDevice));
+	if (int rc = fmt_setup(h)) return rc;
 	h->json_on = true;
 	return 0;
 }
@@ -2195,6 +2307,68 @@ int aisgpu_poll_lines(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, s
 		return AISGPU_EINVAL;
 	}
 	return poll_records(h, ticket, out, cap, n_bytes, n_records, "aisgpu_poll_lines");
+}
+
+namespace {
+
+// Receiver::setChannel's test of a designation letter (Application/Receiver.cpp:103-105): alphanumeric or '?'
+bool channel_letter_ok(char c) { return (c >= 'A' && c <= 'Z') || (c >= 'a' && c <= 'z') || (c >= '0' && c <= '9') || c == '?'; }
+
+// The rules of aisgpu_set_receivers that need no device: "" or the reason.  channel_b is read where a stream has two channels (AB
+// mode, and the FM-discriminator input model in either mode).
+std::string receivers_refusal(const aisgpu_config &c, const aisgpu_receiver *r, int n) {
+	if (!r) return "aisgpu_set_receivers: null receiver table";
+	if (n != c.n_streams) return "aisgpu_set_receivers: " + std::to_string(n) + " receivers for " + std::to_string(c.n_streams) + " streams";
+	const bool two = c.channel_mode != AISGPU_MODE_X || c.model == AISGPU_MODEL_DISCRIMINATOR;
+	for (int s = 0; s < n; s++) {
+		if (!channel_letter_ok(r[s].channel_a)) return "invalid NMEA channel designation: " + std::string(1, r[s].channel_a);
+		if (two && !channel_letter_ok(r[s].channel_b)) return "invalid NMEA channel designation: " + std::string(1, r[s].channel_b);
+	}
+	return "";
+}
+
+} // namespace
+
+int aisgpu_check_receivers(const aisgpu_config *cfg, const aisgpu_receiver *r, int n) {
+	aisgpu_config c;
+	if (!copy_config(cfg, &c)) {
+		g_create_error = "aisgpu_check_receivers: null config or struct_size mismatch";
+		return AISGPU_EINVAL;
+	}
+	const std::string why = receivers_refusal(c, r, n);
+	if (!why.empty()) {
+		g_create_error = why;
+		return AISGPU_EINVAL;
+	}
+	return 0;
+}
+
+int aisgpu_set_receivers(aisgpu_handle *h, const aisgpu_receiver *r, int n) {
+	ENTER(h);
+	std::string why = receivers_refusal(h->given, r, n);
+	if (why.empty() && h->rx_table) why = "aisgpu_set_receivers: a receiver table is already installed";
+	if (why.empty() && h->counters[3] > 0) why = "aisgpu_set_receivers: the engine has been submitted to (install the table before the first submit)";
+	if (!why.empty()) {
+		h->err = why;
+		return AISGPU_EINVAL;
+	}
+	std::vector<Receiver> rx((size_t)n);
+	for (int s = 0; s < n; s++) {
+		rx[s].channel_a = r[s].channel_a;
+		rx[s].channel_b = r[s].channel_b;
+		rx[s].station = r[s].station;
+		rx[s].own_mmsi = r[s].own_mmsi;
+		rx[s].tag_mode = r[s].tag_mode;
+		rx[s].driver = r[s].driver;
+		rx[s].hardware = r[s].hardware ? r[s].hardware : "";
+		rx[s].ipv4 = r[s].ipv4;
+	}
+	h->rx.swap(rx);
+	h->rx_table = true;
+	if (int rc = put_level_rows(h)) return rc;
+	if (h->json_on)
+		if (int rc = fmt_setup(h)) return rc;
+	return 0;
 }
 
 int aisgpu_tap(aisgpu_handle *h, int tap, int stream, int channel, void *dst, size_t dst_bytes, size_t *n_out) {

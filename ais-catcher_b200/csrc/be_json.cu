@@ -1706,13 +1706,14 @@ __global__ void __launch_bounds__(256) k_fmt_groups(const aisgpu_msg *__restrict
 	if (threadIdx.x == 0) total[3] = s_carry - base;
 }
 
-// record i (frame ordinal + i) into the first cap bytes of its slot, the rest of the slot its scratch; its length into len[i]
-__global__ void k_fmt_records(const aisgpu_msg *__restrict__ msgs, int n, const FmtCtx *__restrict__ ctx, long long ordinal,
+// record i (frame ordinal + i) into the first cap bytes of its slot, the rest of the slot its scratch; its length into len[i].  The
+// context is ctx[0], or with per_stream that of the frame's stream (a receiver table)
+__global__ void k_fmt_records(const aisgpu_msg *__restrict__ msgs, int n, const FmtCtx *__restrict__ ctx, int per_stream, long long ordinal,
 							  const long long *__restrict__ groups, char *__restrict__ slots, int slot, int cap, int *__restrict__ len) {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
 	char *s = slots + (size_t)i * slot;
-	len[i] = record(msgs + i, *ctx, ordinal + i, groups[i], s, cap, s + cap, slot - cap);
+	len[i] = record(msgs + i, ctx[per_stream ? msgs[i].stream : 0], ordinal + i, groups[i], s, cap, s + cap, slot - cap);
 }
 
 // Where each record goes: record i is kept when the records of its submit up to and including it fit in cap bytes, and kept
@@ -1815,12 +1816,12 @@ std::string aj_prefix(const aisgpu_tag *tag) {
 	return s;
 }
 
-cudaError_t fmt_launch(const aisgpu_msg *d_msgs, int n, const FmtCtx *d_ctx, long long ordinal, long long groups, long long *d_groups,
+cudaError_t fmt_launch(const aisgpu_msg *d_msgs, int n, const FmtCtx *d_ctx, int per_stream, long long ordinal, long long groups, long long *d_groups,
 					   char *d_slots, int slot, int cap, int *d_len, const int *d_seg, long long budget, long long carry,
 					   long long *d_psum, long long *d_off, int *d_keep, long long *d_total, char *d_text, cudaStream_t st) {
 	if (n <= 0) return cudaSuccess;
 	k_fmt_groups<<<1, 256, 0, st>>>(d_msgs, n, groups, d_groups, d_total);
-	k_fmt_records<<<(n + 127) / 128, 128, 0, st>>>(d_msgs, n, d_ctx, ordinal, d_groups, d_slots, slot, cap, d_len);
+	k_fmt_records<<<(n + 127) / 128, 128, 0, st>>>(d_msgs, n, d_ctx, per_stream, ordinal, d_groups, d_slots, slot, cap, d_len);
 	k_fmt_place<<<1, 256, 0, st>>>(d_len, d_seg, n, budget, carry, d_psum, d_off, d_keep, d_total);
 	k_fmt_copy<<<(n + 7) / 8, 256, 0, st>>>(d_slots, slot, d_keep, d_off, n, d_text);
 	return cudaGetLastError();

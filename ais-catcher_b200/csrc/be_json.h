@@ -30,7 +30,7 @@ int fmt_record_host(const aisgpu_msg *m, const FmtCtx *c, long long ordinal, lon
 
 // The device side of one batch of n published frames (already in d_msgs), four launches on st:
 //   - d_groups[i] = groups + the multi-sentence frames of the batch before frame i, d_total[3] = those of the whole batch;
-//   - record i (frame ordinal + i) into the first cap bytes of the slot d_slots + i * slot (the rest is its scratch), its length
+//   - record i (frame ordinal + i), printed with d_ctx[0] or, with per_stream, d_ctx[stream of frame i], into the first cap bytes of the slot d_slots + i * slot (the rest is its scratch), its length
 //     into d_len[i] (-2: longer than cap);
 //   - the placement: record i is kept when the records of its submit up to and including it fit in budget bytes (d_seg[i] = index
 //     of the first frame of frame i's submit; carry = the bytes the batch's first submit used in earlier batches); d_keep[i] = its
@@ -38,6 +38,6 @@ int fmt_record_host(const aisgpu_msg *m, const FmtCtx *c, long long ordinal, lon
 //     batch's last submit so far (d_psum: scratch, n);
 //   - the kept records packed into d_text.
 // Returns the launch error, if any.
-cudaError_t fmt_launch(const aisgpu_msg *d_msgs, int n, const FmtCtx *d_ctx, long long ordinal, long long groups, long long *d_groups,
+cudaError_t fmt_launch(const aisgpu_msg *d_msgs, int n, const FmtCtx *d_ctx, int per_stream, long long ordinal, long long groups, long long *d_groups,
 					   char *d_slots, int slot, int cap, int *d_len, const int *d_seg, long long budget, long long carry,
 					   long long *d_psum, long long *d_off, int *d_keep, long long *d_total, char *d_text, cudaStream_t st);

@@ -124,7 +124,7 @@ __global__ void __launch_bounds__(PS_THREADS) k_phase_search(const K3Params p) {
 			if (p.tap_dec && active && h == 0) p.tap_dec[inst * p.nsym + t * K3_TS + sl] = bit ? 1.0f : -1.0f;
 		}
 		if (active && h == 0) p.dbits[inst * p.dwords + t] = word;
-		if (active && phase == 0 && p.mode_level) { // ScatterPLL level: ((((0+n0)+n1)+n2)+n3)+n4, then / 5
+		if (active && phase == 0 && row_level(p.level_rows, row)) { // ScatterPLL level: ((((0+n0)+n1)+n2)+n3)+n4, then / 5
 			const float2 *rowt = &mytile[t & 1][half * K3_ROWLEN];
 			for (int sl = h; sl < s_end; sl += 16) {
 				float acc = 0.0f;
@@ -220,6 +220,10 @@ __global__ void __launch_bounds__(32, 28) k_phase_search_ema4b(const K3Params p)
 		max_idx = st.max_idx;
 	}
 	const int nsamp = p.nsym * 5;
+	uint32_t lvl_rows = 0u; // bit r: the frames of tile row r (row r_lo + r) carry the signal level, so its ScatterPLL level is wanted
+#pragma unroll
+	for (int r = 0; r < PS2_TROWS; r++)
+		if (r_lo + r < p.rows && row_level(p.level_rows, r_lo + r)) lvl_rows |= 1u << r;
 	// a tile row is K3_ROWLEN = 5 x 32 samples: five 8-byte copies per lane and row, no index arithmetic beyond the row's base
 	static_assert(K3_ROWLEN == 5 * 32, "tile row = five warp-wide copies");
 	const float2 *rowsrc[PS2_TROWS];
@@ -357,11 +361,11 @@ __global__ void __launch_bounds__(32, 28) k_phase_search_ema4b(const K3Params p)
 		if (p.tap_dec && active) { // decoder input tap: one float per symbol, eight symbols per lane of the instance
 			for (int sx = 8 * q; sx < min(8 * q + 8, s_end); sx++) p.tap_dec[inst * p.nsym + t * K3_TS + sx] = ((word >> sx) & 1u) ? 1.0f : -1.0f;
 		}
-		if (p.mode_level) { // ScatterPLL level: ((((0+n0)+n1)+n2)+n3)+n4, then / 5 (DSP.h:100-106), by the warp that holds the row's phase 0
+		if (lvl_rows) { // ScatterPLL level: ((((0+n0)+n1)+n2)+n3)+n4, then / 5 (DSP.h:100-106), by the warp that holds the row's phase 0
 #pragma unroll
 			for (int r = 0; r < PS2_TROWS; r++) {
 				const long long first = (long long)(r_lo + r) * 5; // the row's phase-0 instance
-				if (first >= inst0 && first < inst0 + PS2_INST && r_lo + r < p.rows && lane < s_end) {
+				if (((lvl_rows >> r) & 1u) && first >= inst0 && first < inst0 + PS2_INST && lane < s_end) {
 					const float2 *rowt = &tile[t & 1][r][lane * 5];
 					float acc = 0.0f;
 #pragma unroll
@@ -435,7 +439,7 @@ __global__ void __launch_bounds__(DK_THREADS) k_decode(const K3Params p) {
 
 	DecCtx ctx;
 	ctx.frame = frames_all[wib] + lane;
-	ctx.mode_level = p.mode_level;
+	ctx.mode_level = row_level(p.level_rows, row);
 	ctx.stride = K3_THREADS;
 	DecState d;
 	const int sidx = row * 5 + (active ? phase : 0);
@@ -648,6 +652,10 @@ __device__ __forceinline__ uint32_t lowmask(int n) { return n >= 32 ? 0xffffffff
 
 // Consumes bits [i0, i1) of the word.  Returns 32, or the index of the bit at which a CRC-valid frame closed (the
 // state is then TRAINING with e = that bit, the frame bits are complete in shared memory, fr_len / fr_level set).
+// The row's level switch (ctx.mode_level) is not read here: a row whose frames carry no level never has its symbol levels computed
+// (the phase search skips it), so they stay the +0 the engine zeroed them with, the level sums +0, and fr_level = +0 / position is
+// the +0 the switch would give.  Read from a register for the whole kernel, the switch pushed k_decode3<2, *> and k_decode10 into
+// spilling.  LEVEL = false (FM rows): the level is never summed and stays +0 alike.
 template <bool LEVEL>
 __device__ __forceinline__ int dk3_run(Dk3 &st, const DecCtx &ctx, uint32_t Bitw, uint32_t E, int i0, int i1, const float *__restrict__ lvl,
 									   int slot0, int phase, int &fr_len, float &fr_level) {
@@ -770,7 +778,7 @@ __device__ __forceinline__ int dk3_run(Dk3 &st, const DecCtx &ctx, uint32_t Bitw
 				i += exit_m + 1;
 				continue;
 			}
-			if (LEVEL && ctx.mode_level) { // level += tag.sample_lvl for every bit in DATAFCS, in order (AIS.h:146-147)
+			if (LEVEL) { // level += tag.sample_lvl for every bit in DATAFCS, in order (AIS.h:146-147)
 				float lv = st.level;
 #pragma unroll
 				for (int m = 0; m < 32; m++) {
@@ -787,7 +795,7 @@ __device__ __forceinline__ int dk3_run(Dk3 &st, const DecCtx &ctx, uint32_t Bitw
 				const int len = newpos - 7;
 				if (len >= 16 && dec_crc16_bytes(ctx, len)) {
 					fr_len = len;
-					fr_level = ctx.mode_level ? __fdiv_rn(st.level, (float)newpos) : 0.0f;
+					fr_level = __fdiv_rn(st.level, (float)newpos);
 					st.pos = newpos;
 					return i - 1;
 				}
@@ -821,7 +829,7 @@ __global__ void __launch_bounds__(DK3_WARPS * 32) k_decode3(const K3Params p) {
 
 	DecCtx ctx;
 	ctx.frame = frames_all[wib] + lane;
-	ctx.mode_level = p.mode_level;
+	ctx.mode_level = 1; // not read by dk3_run: a row without level has all-zero symbol levels (see there)
 	ctx.stride = K3_THREADS;
 	DecState d;
 	const int sidx = active ? row * 5 + phase : 0;
@@ -1007,7 +1015,7 @@ __global__ void __launch_bounds__(DK3_WARPS * 32) k_decode10(const K3Params p) {
 
 	DecCtx ctx;
 	ctx.frame = frames_all[wib] + lane;
-	ctx.mode_level = p.mode_level;
+	ctx.mode_level = 1; // not read by dk3_run: a row without level has all-zero symbol levels (see there)
 	ctx.stride = K3_THREADS;
 	DecState d;
 	const int sidx = active ? row * 10 + ph10 : 0;

@@ -40,7 +40,8 @@ struct V2Params {
 	uint32_t *dec_data; // [DEC_WORDS][rows * 6]
 	FrameRec *ring;
 	unsigned long long *ring_head, ring_limit;
-	int ring_cap, chunk, blk, mode_level;
+	int ring_cap, chunk, blk;
+	const uint32_t *level_rows;
 	const float2 *omega_g;
 	float w_train, w_track;
 	float2 *tap_fc, *tap_coh; // optional [rows][nproc * 512]: the blocks this launch processed
@@ -90,7 +91,7 @@ __global__ void __launch_bounds__(V2_WARPS * 32, 4) k_v2_engine(const V2Params p
 	}
 	DecCtx ctx;
 	ctx.frame = frames + (lane < 6 ? lane : 0);
-	ctx.mode_level = p.mode_level;
+	ctx.mode_level = row_level(p.level_rows, row);
 	ctx.stride = 8;
 	DecState d;
 	d.state = ST_TRAINING; d.lastBit = 0; d.prev = 0; d.position = 0; d.one_seq = 0; d.level = 0.f; d.start_idx = 0;
@@ -392,7 +393,7 @@ cudaError_t launch_v2_engine(const float2 *Cbuf, long long c_stride, int c_begin
 	V2Params p;
 	p.Cbuf = Cbuf; p.c_stride = c_stride; p.c_begin = c_begin; p.nproc = nproc; p.rows = rows; p.st = st; p.dec = dec; p.dec_data = dec_data;
 	p.ring = out.ring; p.ring_head = out.ring_head; p.ring_limit = out.ring_limit; p.ring_cap = out.ring_cap; p.chunk = out.chunk; p.blk = out.blk;
-	p.mode_level = out.mode_level;
+	p.level_rows = out.level_rows;
 	p.omega_g = omega_g; p.w_train = w_train; p.w_track = w_track; p.tap_fc = tap_fc; p.tap_coh = tap_coh; p.tap_fmf = tap_fmf; p.tap_stride = tap_stride;
 	k_v2_engine<<<(rows + V2_WARPS - 1) / V2_WARPS, V2_WARPS * 32, V2_WARPS * V2_WARP_BYTES, s>>>(p);
 	return cudaGetLastError();

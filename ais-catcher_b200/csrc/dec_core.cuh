@@ -8,7 +8,7 @@ namespace aisgpu {
 
 struct DecCtx {
 	uint32_t *frame; // shared memory, word w of this thread at frame[w * stride]
-	int mode_level;
+	int mode_level;  // the row's frames carry the signal level (row_level)
 	int stride;      // threads sharing the frame array (32 in the decoder kernels)
 };
 

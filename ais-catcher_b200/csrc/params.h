@@ -117,8 +117,11 @@ struct FrameOut {
 	int ring_cap;
 	int chunk;                     // ordinal of the caller's submit
 	int blk;                       // ordinal of the front-end block
-	int mode_level;                // tag_mode & 1: frames carry the signal level
+	const uint32_t *level_rows;    // bit r of word r >> 5: row r's frames carry the signal level (its stream's tag_mode & 1)
 };
+
+// Whether row r's frames carry the signal level (FrameOut::level_rows)
+__host__ __device__ __forceinline__ int row_level(const uint32_t *level_rows, int r) { return (int)((level_rows[r >> 5] >> (r & 31)) & 1u); }
 
 
 struct K3Params {
@@ -151,7 +154,7 @@ struct K3Params {
 	int ring_cap;
 	int chunk;
 	int blk;
-	int mode_level;
+	const uint32_t *level_rows; // FrameOut::level_rows
 	// tag.ppm lookup (ModelDefault): block index of a sample = (abs_idx - blk_abs0) >> 9
 	const int *stepidx;
 	const float *ppmtab;
@@ -237,7 +240,7 @@ cudaError_t sym_init(const float *ps_cos8, const float *ps_sin8, const uint32_t 
 cudaError_t launch_phase_search(const K3Params &p, cudaStream_t s);
 cudaError_t launch_decode(int model, int decoder, int rpw, const K3Params &p, cudaStream_t s);
 cudaError_t launch_decode10(int rpw, const K3Params &p, cudaStream_t s);
-// out.mode_level is not read: k_base always sums the level (its sample levels are 0)
+// out.level_rows is not read: k_base always sums the level (its sample levels are 0)
 cudaError_t launch_base(const float *Ef, long long e_stride, int e_begin, int n, int rows, PllState *pll, DecState *dec, uint32_t *dec_data,
                         const FrameOut &out, float *tap_dec, int *tap_cnt, cudaStream_t s);
 

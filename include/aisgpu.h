@@ -33,7 +33,8 @@ extern "C" {
 #endif
 
 /* 3 since the engine groups; later additions are new entry points only (the full AIS JSON: aisgpu_msg_json_full, aisgpu_json_enable,
- * aisgpu_poll_json; the output records: aisgpu_msg_format, aisgpu_lines_enable, aisgpu_poll_lines), so the number callers check
+ * aisgpu_poll_json; the output records: aisgpu_msg_format, aisgpu_lines_enable, aisgpu_poll_lines; the receivers:
+ * aisgpu_set_receivers, aisgpu_check_receivers), so the number callers check
  * against stays 3.  A caller that needs those entry points looks them up
  * (dlsym) instead of relying on the number. */
 #define AISGPU_ABI_VERSION 3
@@ -112,10 +113,10 @@ typedef struct aisgpu_config {
 	int32_t ps_ema;             /* -go PS_EMA   (Model.cpp:583-585), default 1 */
 	int32_t afc_wide;           /* -go AFC_WIDE (Model.cpp:586-588), default 1 */
 	int32_t droop;              /* -go DROOP    (Model.cpp:384-386), default 1 */
-	char channel_a, channel_b;  /* CH1/CH2 of buildModel (Model.cpp:547-548), default 'A','B' */
-	int32_t station;            /* Model::station  (Model.h:79) */
-	int32_t own_mmsi;           /* Model::own_mmsi (Model.h:80): sentences of this MMSI read !AIVDO */
-	uint32_t tag_mode;          /* TAG::mode (Common.h:242): bit0 = signal level, default 3 */
+	char channel_a, channel_b;  /* CH1/CH2 of buildModel (Model.cpp:547-548), default 'A','B' (a receiver table overrides: aisgpu_set_receivers) */
+	int32_t station;            /* Model::station  (Model.h:79) (a receiver table overrides) */
+	int32_t own_mmsi;           /* Model::own_mmsi (Model.h:80): sentences of this MMSI read !AIVDO (a receiver table overrides) */
+	uint32_t tag_mode;          /* TAG::mode (Common.h:242): bit0 = signal level, default 3 (a receiver table overrides) */
 	int32_t device;             /* CUDA device ordinal */
 	int32_t enable_taps;        /* keep intermediates readable through aisgpu_tap() */
 	int32_t max_frames;         /* capacity of the device frame ring = frames that may wait between two polls (0 = default) */
@@ -267,7 +268,9 @@ int aisgpu_build_nmea(aisgpu_msg *m, int own_mmsi, int *seq);
 /* ---- Formats either side of the path (SURVEY.md 8f rank 4) ---- */
 
 /* The TAG / receiver fields the reference's outputs print next to a message (Source/Library/Common.h:218-250 TAG;
- * Message::rxtime/toa/station, Message.h:60-75).  level and ppm are taken from the aisgpu_msg. */
+ * Message::rxtime/toa/station, Message.h:60-75).  level and ppm are taken from the aisgpu_msg.  On an engine with a receiver table
+ * (aisgpu_set_receivers), the records of stream s take driver, hardware, mode, ipv4 and station from the stream's receiver; version,
+ * status, rxtime_us, toa_us, include_ssl, uuid and suffix stay the output's, for every stream. */
 typedef struct aisgpu_tag {
 	int32_t version;      /* TAG::version */
 	int32_t driver;       /* TAG::driver (Type enum as int) */
@@ -387,6 +390,47 @@ int aisgpu_msg_format(const aisgpu_msg *m, const aisgpu_tag *tag, int msgformat,
  * strings. */
 int aisgpu_lines_enable(aisgpu_handle *h, int msgformat, const aisgpu_tag *tag, int max_bytes_per_submit);
 int aisgpu_poll_lines(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, size_t *n_bytes, int *n_records);
+
+/* ---- Receivers: one per stream (the reference's repeated receiver objects, Application/Config.cpp:421) ----
+ *
+ * Every stream of a batch is a receiver of its own.  Without a table every stream takes the config's channel_a / channel_b, station,
+ * own_mmsi and tag_mode, and every record the engine formats takes the aisgpu_tag of aisgpu_lines_enable / aisgpu_json_enable.
+ * aisgpu_set_receivers installs r[0 .. n_streams - 1]: from then on stream s behaves as if its engine had been created with r[s]'s
+ * channel_a / channel_b, station, own_mmsi and tag_mode --
+ *   - its frames carry r[s].channel_a / channel_b (aisgpu_msg.channel) and read !AIVDO for r[s].own_mmsi (Receiver::setOwnMMSI,
+ *     Receiver.cpp:221);
+ *   - tag_mode bit 0 decides, per stream, whether its frames carry the signal level and convert it to dB (AIS.cpp:73-75): the back
+ *     ends read a level switch per 48 kHz row;
+ * -- and its records (aisgpu_poll_lines, aisgpu_poll_json) are printed with the output's tag whose station, driver, hardware, mode
+ * (= tag_mode) and ipv4 are r[s]'s (Message::setOrigin, Message.h:300-306; the TAG of -M DTM, Receiver.cpp:26-66).  version, status,
+ * rxtime_us, toa_us, include_ssl, uuid and suffix stay the output's, and so do the COMMUNITY_HUB and NMEA_TAG counters (per engine).
+ * counters[5] / [6] keep counting each stream's first and second channel, whatever its letters.  So the records expected for stream s
+ * are exactly aisgpu_msg_format(frame, tag of s, ...).
+ *
+ * Rules (AISGPU_EINVAL with the reason in aisgpu_last_error(h), the handle untouched): n == n_streams; before the first submit; at
+ * most once.  Every letter the engine prints must pass Receiver::setChannel's test (Receiver.cpp:103-105), alphanumeric or '?', else
+ * the reason is the reference's "invalid NMEA channel designation: <c>"; channel_b is only read where a stream has two channels (AB
+ * mode, and AISGPU_MODEL_DISCRIMINATOR in both modes).  It may come before or after aisgpu_lines_enable / aisgpu_json_enable: the
+ * per-stream record contexts are made when both are known.  A group member takes a table of its own; the leader's does not reach
+ * it.  hardware is copied (NULL: "").
+ *
+ * Memory: a level bit per row (always).  With a table and a format enabled, the device holds one record context (96 bytes) and the
+ * stream's hardware name and full-JSON prefix (about 100 bytes plus the name) per stream, and every record slot (above) is sized for
+ * the longest hardware name and prefix among the streams. */
+typedef struct aisgpu_receiver {
+	char channel_a, channel_b; /* the receiver's NMEA designation (CH1 / CH2 of buildModel); X mode: channel_b unused */
+	int32_t station;           /* Model::station: NMEA_TAG s:, station_id, FULL's ID */
+	int32_t own_mmsi;          /* Model::own_mmsi: this MMSI's sentences read !AIVDO */
+	uint32_t tag_mode;         /* TAG::mode of the receiver: bit 0 level in dB + signalpower / ppm printed, bit 1 time, bit 2 country */
+	int32_t driver;            /* TAG::driver */
+	const char *hardware;      /* TAG::hardware, may be NULL ("") */
+	uint32_t ipv4;             /* TAG::ipv4 */
+} aisgpu_receiver;
+
+int aisgpu_set_receivers(aisgpu_handle *h, const aisgpu_receiver *r, int n);
+/* The rules of aisgpu_set_receivers that need no device, for an engine created with *cfg (struct_size as for aisgpu_create): 0, or
+ * AISGPU_EINVAL with the reason in aisgpu_last_error(NULL). */
+int aisgpu_check_receivers(const aisgpu_config *cfg, const aisgpu_receiver *r, int n);
 
 /* == AIS::Message::getBinaryNMEA(out, tag, crc) (Message.cpp:277-396): 0xAC 0x00 framed, byte-stuffed binary record with an
  * optional CRC-16 (Helper.cpp:42-57).  Returns the bytes written, 0 when the reference would emit nothing. Host-only. */
