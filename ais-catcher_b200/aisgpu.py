@@ -26,7 +26,8 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_msg_json", "aisgpu_msg_binary", "aisgpu_feed_files", "aisgpu_check_device_batch", "aisgpu_attach",
            "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files",
            "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json", "aisgpu_msg_format", "aisgpu_lines_enable",
-           "aisgpu_poll_lines", "aisgpu_set_receivers", "aisgpu_check_receivers"]
+           "aisgpu_poll_lines", "aisgpu_set_receivers", "aisgpu_check_receivers",
+           "aisgpu_set_tuning", "aisgpu_check_tuning", "aisgpu_tune_restate"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 # message formats: positions in the reference's enum class MessageFormat (MSGFORMAT of its outputs); include/aisgpu.h describes each record
@@ -89,6 +90,35 @@ def check_receivers(receivers, **engine):
     rc = lib.aisgpu_check_receivers(C.byref(make_config(**engine)), receiver_table(receivers), len(receivers))
     if rc:
         raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode("latin-1")))
+
+
+def _offsets(offsets):
+    return (C.c_int32 * max(len(offsets), 1))(*[int(f) for f in offsets])
+
+
+def check_tuning(offsets, **engine):
+    """aisgpu_check_tuning (no GPU needed): the rules of Engine.set_tuning for an engine of keyword arguments `engine`.
+    Raises with the reason if the offsets (Hz, one per stream) would be refused."""
+    lib = load()
+    rc = lib.aisgpu_check_tuning(C.byref(make_config(**engine)), _offsets(offsets), len(offsets))
+    if rc:
+        raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode("latin-1")))
+
+
+def tune_restate(fmt, sample_rate, offset_hz, first_sample, samples):
+    """aisgpu_tune_restate: one stream's samples in format fmt (a numpy array of the format's layout: complex64 for CF32, bytes
+    (u)int8 / int16 pairs, float32 for F32_FS4, uint32 triples for DC16H), samples first_sample .. of the stream, mixed by
+    offset_hz -> complex64 array: what a tuned engine's rows after the tune hold."""
+    lib = load()
+    a = np.ascontiguousarray(samples)
+    bps = {FMT_CF32: 8, FMT_CU8: 2, FMT_CS8: 2, FMT_CS16: 4, FMT_F32_FS4: 4, FMT_DC16H: 12}[fmt]
+    n = a.nbytes // bps
+    out = np.empty(n, np.complex64)
+    rc = lib.aisgpu_tune_restate(int(fmt), int(sample_rate), int(offset_hz), int(first_sample), a.ctypes.data_as(C.c_void_p), n,
+                                 out.ctypes.data_as(C.c_void_p))
+    if rc:
+        raise AisGpuError("aisgpu_tune_restate rc=%d" % rc)
+    return out
 
 
 MSG_FN = C.CFUNCTYPE(None, C.POINTER(MsgStruct), C.c_int, C.c_void_p)
@@ -177,6 +207,10 @@ def load():
     if hasattr(lib, "aisgpu_set_receivers"):  # absent from libraries built before the receiver tables (AISGPU_LIB)
         lib.aisgpu_set_receivers.argtypes = [C.c_void_p, C.POINTER(Receiver), C.c_int]
         lib.aisgpu_check_receivers.argtypes = [C.POINTER(Config), C.POINTER(Receiver), C.c_int]
+    if hasattr(lib, "aisgpu_set_tuning"):  # absent from libraries built before the tuning tables (AISGPU_LIB)
+        lib.aisgpu_set_tuning.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
+        lib.aisgpu_check_tuning.argtypes = [C.POINTER(Config), C.POINTER(C.c_int32), C.c_int]
+        lib.aisgpu_tune_restate.argtypes = [C.c_int, C.c_int, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -521,6 +555,11 @@ class Engine:
         printed with its station, driver, hardware, mode and ipv4."""
         self._receivers = receiver_table(receivers)  # copied by the library; kept anyway
         self._chk(self.lib.aisgpu_set_receivers(self.h, self._receivers, len(receivers)))
+
+    def set_tuning(self, offsets):
+        """aisgpu_set_tuning: one offset in Hz per stream (the channel pair's centre, or in X mode the channel, relative to the
+        capture's centre), before the first submit and at most once.  Each submit is then mixed on the GPU so that it lands at 0 Hz."""
+        self._chk(self.lib.aisgpu_set_tuning(self.h, _offsets(offsets), len(offsets)))
 
     def poll_lines(self, ticket=None, cap=1 << 20):
         """aisgpu_poll_lines: (bytes, number of records) of the frames of the submits up to ticket (None: all), in frame order."""

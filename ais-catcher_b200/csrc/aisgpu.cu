@@ -147,6 +147,7 @@ struct aisgpu_handle {
 	FeParams fe_pre;
 	long long msg_chunk = 0; // ordinal of the caller's submit (what frames are tagged with)
 	int obps = 8;            // bytes per sample of the caller's format (bps: of what the front end proper reads)
+	int pbps = 8;            // bytes per sample of what the pre-stage reads: the caller's format, CF32 behind the tune
 	int inner_max = 0;       // longest block the front end proper can be handed
 	int use_fdc = 0;
 	int fp_ds = 0; // integer CIC front end (DS_UINT16 x 4, DSP.cpp:499-665): CU8 @1536K with -go FP_DS on
@@ -261,6 +262,15 @@ struct aisgpu_handle {
 	std::vector<int> seq; // per-stream multi-sentence sequence id (Message.cpp:28-39 is process-global in the reference)
 	std::vector<Receiver> rx; // per stream: the config's fields, or the receiver aisgpu_set_receivers installed
 	bool rx_table = false;    // aisgpu_set_receivers has been called: the records take the receivers' TAG fields
+	// The per-stream digital tune (aisgpu_set_tuning, tune.cu).  With a table every submit first runs k_tune on fe_stream: the
+	// caller's samples, converted and mixed by each stream's offset, into d_tune [n_streams][tune_stride] as CF32, which everything
+	// behind it then reads as a CF32 input (src_fmt); behind a resampler with no CIC stage (kA = 0) k_tune writes D0 directly and is
+	// the pre-stage's conversion.  Without a table nothing of this is allocated or launched.
+	bool tuned = false;
+	float2 *d_tune = nullptr, *d_tune_tab = nullptr;
+	long long tune_stride = 0;
+	int *d_tune_fk = nullptr;
+	int tune_ctas = 0;
 	// last-submit geometry (for taps)
 	int last_n = 0, last_n48 = 0, last_nE = 0, last_nsym = 0, last_launches = 0;
 	uint64_t counters[8] = { 0 };
@@ -439,6 +449,12 @@ int put_level_rows(aisgpu_handle *h) {
 
 bool has_cic(const aisgpu_handle *h) { return h->pre_us || h->kA > 0; }
 
+// The format the first stage reads: the caller's, or the CF32 rows of the tune (aisgpu_set_tuning)
+int src_fmt(const aisgpu_handle *h) { return h->tuned ? AISGPU_FMT_CF32 : h->cfg.format; }
+
+// A tuned engine whose CIC stage would only convert (a resampler behind no CIC stage): the tune writes D0 in its place
+bool tune_into_d0(const aisgpu_handle *h) { return h->tuned && h->pre_us && h->kA == 0; }
+
 // The CIC stage's warm-up history for h->kA stages (5 input samples per stage and level), rounded up to a whole number of
 // super-steps of the streaming kernel (and even tiles at every level)
 void plan_cic(aisgpu_handle *h) {
@@ -467,7 +483,7 @@ int plan_frontend_x(aisgpu_handle *h) {
 	while (bucket < sr) bucket *= 2;
 	h->kA = 0;
 	h->fp_ds = 0;
-	h->in_fmt = h->cfg.format;
+	h->in_fmt = src_fmt(h);
 	h->k = bucket == 192000 ? 2 : (bucket == 96000 ? 1 : 0);
 	if (bucket != sr) plan_upsample(h, sr, bucket); // "sample rate ...K upsampled to ...K." (Model.cpp:58-59)
 	h->use_fdc = (h->cfg.droop && h->k > 0) ? 1 : 0;
@@ -498,7 +514,7 @@ int plan_frontend_disc(aisgpu_handle *h) {
 	h->kA = 0;
 	h->k = 0;
 	h->fp_ds = 0;
-	h->in_fmt = h->cfg.format;
+	h->in_fmt = src_fmt(h);
 	if (sr != 48000) plan_upsample(h, sr, 48000); // US.setParams(sample_rate, 48000) (Model.cpp:722-728)
 	h->use_fdc = 0;
 	h->P = 0; // the split has no filter state: no warm-up history
@@ -534,7 +550,7 @@ int plan_frontend(aisgpu_handle *h) {
 	const bool interp = bucket != sr; // "sample rate ...K upsampled to ...K." (Model.cpp:146-147)
 	h->kA = 0;
 	h->fp_ds = 0;
-	h->in_fmt = h->cfg.format;
+	h->in_fmt = src_fmt(h);
 	int k_total = 0;
 	if (bucket == 288000 || bucket == 576000 || bucket == 1152000 || bucket == 2304000) {
 		// [kA x Downsample2CIC5 ->] [Upsample ->] DownsampleKFilter(BlackmanHarris_28_3, 3) -> ROT, no droop filter
@@ -1272,7 +1288,7 @@ int pre_cic(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	pp.in = dev_in;
 	pp.tail = h->d_raw_tail[h->raw_tail_cur];
 	pp.in_stride = stride;
-	pp.format = h->cfg.format;
+	pp.format = src_fmt(h);
 	pp.k = h->kA;
 	pp.N = N;
 	pp.P = h->PA;
@@ -1282,7 +1298,7 @@ int pre_cic(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	pp.D0 = h->d_D0;
 	pp.d0_stride = h->d0_stride;
 	pp.d0_off = 2;
-	if (int rc = launch_cic(h, pp, h->cfg.format, h->obps, h->kA, true)) return rc;
+	if (int rc = launch_cic(h, pp, src_fmt(h), h->pbps, h->kA, true)) return rc;
 	h->last_launches++;
 	return 0;
 }
@@ -1351,7 +1367,7 @@ int pre_dsk(aisgpu_handle *h, const void *src, long long stride, int N) {
 	const int first = h->dsk_first;
 	const int n_out = first < N ? (N - first + 2) / 3 : 0;
 	if (n_out > 0) {
-		CU(launch_dsk(fe_fmt_id(cf32 ? AISGPU_FMT_CF32 : h->cfg.format), src, stride, tail, 32, first, n_out, B, r.d, r.stride, r.produced, r.cap, h->fe_stream));
+		CU(launch_dsk(fe_fmt_id(cf32 ? AISGPU_FMT_CF32 : src_fmt(h)), src, stride, tail, 32, first, n_out, B, r.d, r.stride, r.produced, r.cap, h->fe_stream));
 		h->last_launches++;
 	}
 	h->dsk_first = first + 3 * n_out - N;
@@ -1440,10 +1456,35 @@ int check_placement(aisgpu_handle *h, const void *dev, int64_t stride) {
 
 int mark_ticket(aisgpu_handle *h, long long t);
 
+// The tune stage (aisgpu_set_tuning): the caller's N samples per stream, sample 0 being sample counters[2] of every stream, converted
+// and mixed into d_tune (or into D0, tune_into_d0); what follows reads d_tune in place of the caller's rows.
+int tune_input(aisgpu_handle *h, const void *&dev_in, long long &stride, int N) {
+	TuneParams p;
+	p.in = dev_in;
+	p.in_stride = stride;
+	p.out = h->d_tune ? h->d_tune : h->d_D0;
+	p.out_stride = h->d_tune ? h->tune_stride : h->d0_stride;
+	p.out_off = h->d_tune ? 0 : 2;
+	p.N = N;
+	p.B = h->cfg.n_streams;
+	p.fs = h->cfg.sample_rate;
+	p.tab_len = tune_table_len(p.fs);
+	p.first = (long long)h->counters[2];
+	p.fk = h->d_tune_fk;
+	p.tab = h->d_tune_tab;
+	CU(launch_tune(p, fe_fmt_id(h->cfg.format), h->tune_ctas, h->fe_stream));
+	h->last_launches++;
+	dev_in = h->d_tune;
+	stride = h->tune_stride;
+	return 0;
+}
+
 // The caller's Receive(): N samples per stream in the caller's format.
 int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	if (int rc = check_outer(h, N)) return rc;
 	h->last_launches = 0;
+	if (h->tuned)
+		if (int rc = tune_input(h, dev_in, stride, N)) return rc;
 	h->msg_chunk = (long long)h->counters[3];
 	for (aisgpu_handle *m : h->members) {
 		m->last_launches = 0;
@@ -1456,15 +1497,15 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 	else {
 		h->us_ring.last = h->us_ring.produced;
 		h->dsk_ring.last = h->dsk_ring.produced;
-		if (has_cic(h))
+		if (has_cic(h) && !tune_into_d0(h))
 			if (int rc = pre_cic(h, dev_in, stride, N)) return rc;
 		if (h->pre_us) {
 			if (int rc = pre_upsample(h, N)) return rc;
 		}
 		else if (int rc = has_cic(h) ? pre_dsk(h, h->d_D0 + 2, h->d0_stride, N >> h->kA) : pre_dsk(h, dev_in, stride, N)) return rc;
-		{ // raw-format history of the pre-stage for the next submit
+		if (!tune_into_d0(h)) { // raw-format history of the pre-stage for the next submit
 			const int cur = h->raw_tail_cur, tl = raw_tail_len(h);
-			CU(launch_tail_update(h->d_raw_tail[cur ^ 1], h->d_raw_tail[cur], dev_in, stride * h->obps, (long long)N * h->obps, tl * h->obps, h->cfg.n_streams, h->fe_stream));
+			CU(launch_tail_update(h->d_raw_tail[cur ^ 1], h->d_raw_tail[cur], dev_in, stride * h->pbps, (long long)N * h->pbps, tl * h->pbps, h->cfg.n_streams, h->fe_stream));
 			h->raw_tail_cur = cur ^ 1;
 			h->last_launches++;
 		}
@@ -1846,6 +1887,7 @@ static int create_impl(aisgpu_handle *h) {
 	h->cfg.max_chunk_samples = maxN;
 	h->rows = rows_of(h);
 	h->obps = bytes_per_sample(c.format);
+	h->pbps = h->obps;
 	h->bps = bytes_per_sample(h->in_fmt);
 	h->inner_max = h->pre_dsk ? h->blk : (h->pre_us ? (maxN >> h->kA) : maxN);
 	h->max_n48 = h->inner_max >> ((h->xmode || h->disc) ? k : k + 1);
@@ -2368,6 +2410,89 @@ int aisgpu_set_receivers(aisgpu_handle *h, const aisgpu_receiver *r, int n) {
 	if (int rc = put_level_rows(h)) return rc;
 	if (h->json_on)
 		if (int rc = fmt_setup(h)) return rc;
+	return 0;
+}
+
+namespace {
+
+// The rules of aisgpu_set_tuning that need no device: "" or the reason.  fp_ds: the engine runs the integer CIC front end.
+std::string tuning_refusal(const aisgpu_config &c, bool fp_ds, const int32_t *f, int n) {
+	if (!f) return "aisgpu_set_tuning: null offset table";
+	if (n != c.n_streams) return "aisgpu_set_tuning: " + std::to_string(n) + " offsets for " + std::to_string(c.n_streams) + " streams";
+	if (c.model == AISGPU_MODEL_DISCRIMINATOR)
+		return "aisgpu_set_tuning: the FM-discriminator input model reads I and Q as two real audio channels: there is nothing to tune";
+	if (fp_ds) return "aisgpu_set_tuning: FP_DS on: the integer front end reads the caller's CU8 samples directly and cannot take tuned ones";
+	const long long fs = c.sample_rate;
+	for (int s = 0; s < n; s++)
+		if (2 * (long long)f[s] <= -fs || 2 * (long long)f[s] >= fs)
+			return "aisgpu_set_tuning: stream " + std::to_string(s) + ": offset " + std::to_string(f[s]) +
+				   " Hz must lie strictly between -fs/2 and fs/2 (fs = " + std::to_string(fs) + ")";
+	return "";
+}
+
+} // namespace
+
+int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int n) {
+	aisgpu_config c;
+	if (!copy_config(cfg, &c)) {
+		g_create_error = "aisgpu_check_tuning: null config or struct_size mismatch";
+		return AISGPU_EINVAL;
+	}
+	// plan_frontend's FP_DS condition: the exact 1536K bucket of AB mode fed CU8
+	const bool fp_ds = c.fp_ds && c.channel_mode == AISGPU_MODE_AB && c.model != AISGPU_MODEL_DISCRIMINATOR && c.sample_rate == 1536000 &&
+					   c.format == AISGPU_FMT_CU8;
+	const std::string why = tuning_refusal(c, fp_ds, offset_hz, n);
+	if (!why.empty()) {
+		g_create_error = why;
+		return AISGPU_EINVAL;
+	}
+	return 0;
+}
+
+int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) {
+	ENTER(h);
+	std::string why = tuning_refusal(h->given, h->fp_ds != 0, offset_hz, n);
+	if (why.empty() && h->member)
+		why = "aisgpu_set_tuning: this engine is a member of a group and reads its leader's front end: install the table on the leader";
+	if (why.empty() && h->tuned) why = "aisgpu_set_tuning: a tuning table is already installed";
+	if (why.empty() && h->counters[3] > 0) why = "aisgpu_set_tuning: the engine has been submitted to (install the table before the first submit)";
+	if (!why.empty()) {
+		h->err = why;
+		return AISGPU_EINVAL;
+	}
+	// Everything behind the tune reads CF32: plan the front end again for it (it passed for the caller's format at creation, and the
+	// plan only differs in the format it reads and the warm-up history that follows from it), and give the warm-up histories CF32 size.
+	const int B = h->cfg.n_streams, fs = h->cfg.sample_rate;
+	h->tuned = true;
+	if (int rc = plan_frontend(h)) return poison(h, rc == AISGPU_EINVAL ? AISGPU_ECUDA : rc);
+	h->bps = bytes_per_sample(h->in_fmt);
+	h->pbps = bytes_per_sample(AISGPU_FMT_CF32);
+	for (int i = 0; i < 2; i++) {
+		dfree(h, h->d_tail[i]);
+		if (h->P)
+			if (int rc = dalloc(h, &h->d_tail[i], (size_t)B * h->P * h->bps)) return poison(h, rc);
+		if (h->d_raw_tail[i]) {
+			dfree(h, h->d_raw_tail[i]);
+			if (int rc = dalloc(h, &h->d_raw_tail[i], (size_t)B * raw_tail_len(h) * h->pbps)) return poison(h, rc);
+		}
+	}
+	if (!tune_into_d0(h)) {
+		h->tune_stride = h->cfg.max_chunk_samples; // a multiple of the granule: even, so every CF32 row is 16-byte aligned
+		if (int rc = dalloc(h, &h->d_tune, (size_t)B * h->tune_stride)) return poison(h, rc);
+	}
+	std::vector<float2> tab((size_t)tune_table_len(fs));
+	tune_tables(fs, tab.data());
+	std::vector<int> fk((size_t)B);
+	for (int s = 0; s < B; s++) fk[s] = offset_hz[s] < 0 ? offset_hz[s] + fs : offset_hz[s];
+	if (int rc = dalloc(h, &h->d_tune_tab, tab.size())) return poison(h, rc);
+	if (int rc = dalloc(h, &h->d_tune_fk, fk.size())) return poison(h, rc);
+	CU(cudaMemcpyAsync(h->d_tune_tab, tab.data(), tab.size() * sizeof(float2), cudaMemcpyHostToDevice, h->stream));
+	CU(cudaMemcpyAsync(h->d_tune_fk, fk.data(), fk.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+	CU(cudaStreamSynchronize(h->stream));
+	// k_tune keeps the tables in shared memory (at most 56.3 KB): four CTAs per SM, each walking many segments
+	int sms = 0;
+	CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->cfg.device));
+	h->tune_ctas = 4 * sms;
 	return 0;
 }
 

@@ -34,7 +34,8 @@ extern "C" {
 
 /* 3 since the engine groups; later additions are new entry points only (the full AIS JSON: aisgpu_msg_json_full, aisgpu_json_enable,
  * aisgpu_poll_json; the output records: aisgpu_msg_format, aisgpu_lines_enable, aisgpu_poll_lines; the receivers:
- * aisgpu_set_receivers, aisgpu_check_receivers), so the number callers check
+ * aisgpu_set_receivers, aisgpu_check_receivers; the tuning: aisgpu_set_tuning, aisgpu_check_tuning, aisgpu_tune_restate), so the
+ * number callers check
  * against stays 3.  A caller that needs those entry points looks them up
  * (dlsym) instead of relying on the number. */
 #define AISGPU_ABI_VERSION 3
@@ -431,6 +432,39 @@ int aisgpu_set_receivers(aisgpu_handle *h, const aisgpu_receiver *r, int n);
 /* The rules of aisgpu_set_receivers that need no device, for an engine created with *cfg (struct_size as for aisgpu_create): 0, or
  * AISGPU_EINVAL with the reason in aisgpu_last_error(NULL). */
 int aisgpu_check_receivers(const aisgpu_config *cfg, const aisgpu_receiver *r, int n);
+
+/* ---- Tuning: a digital tune per stream (DESIGN.md 7d) ----
+ *
+ * Without a table the engine takes each capture as centred where the reference tunes its receiver: AB mode expects the channel pair
+ * at -25 / +25 kHz (162.000 MHz for A/B, 156.800 MHz for C/D), X mode its channel at 0 Hz.  aisgpu_set_tuning gives stream s an
+ * integer offset offset_hz[s]: the frequency of what must land at 0 Hz, relative to the capture's centre -- the pair's centre in AB
+ * mode, the channel in X mode.  From then on every submit first mixes each stream to 0 Hz on the GPU (one read of the input and one
+ * CF32 write per sample), and the rest of the engine runs unchanged on those rows, as on a CF32 input: stream s then yields exactly
+ * the frames (and AISGPU_TAP_C rows, and channel dump) of an untuned engine fed aisgpu_tune_restate(format, sample_rate,
+ * offset_hz[s], 0, its whole input) as CF32 -- which is what the reference yields on that signal.  A stream whose offset is 0 is
+ * converted only, never multiplied: its frames are those of an untuned engine on its raw input, bit for bit.  Host submits, device
+ * batches (any stride and base aisgpu_submit_device takes), aisgpu_feed_files and aisgpu_feed_wav_files all go through the tune.
+ * A group leader's table tunes the rows its whole group reads.
+ *
+ * Rules (AISGPU_EINVAL with the reason in aisgpu_last_error(h), the handle untouched): n == n_streams; before the first submit; at most
+ * once; -sample_rate/2 < offset_hz[s] < sample_rate/2.  Refused outright: AISGPU_MODEL_DISCRIMINATOR (its I and Q are two real audio
+ * channels: nothing to tune), an engine that runs the FP_DS integer front end (it reads CU8 directly), and a group member (its front
+ * end is the leader's).
+ *
+ * Memory: the tables (about 36 KB at 1536 kS/s, 56 KB at 12.288 MS/s), and n_streams x max_chunk_samples CF32 samples of scratch,
+ * except behind a resampler with no CIC stage in front of it, where the tune writes the resampler's input directly. */
+int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n);
+/* The rules of aisgpu_set_tuning that need no device, for an engine created with *cfg: 0, or AISGPU_EINVAL with the reason in
+ * aisgpu_last_error(NULL). */
+int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int n);
+/* The definition of the tune, on the host: n samples of one stream in `format` (samples first_sample .. first_sample + n - 1 of it)
+ * -> n CF32 samples.  Sample m converts as the reference's ConvertRAW does (F32_FS4's 1, j, -1, -j pattern indexed by m) to v; with
+ * f = offset_hz and fs = sample_rate, k = ((m mod fs) * f) mod fs in [0, fs) (int64), k = a * 4096 + b, and
+ *   p = T_hi[a] * T_lo[b],  T_hi[a] = exp(2 pi i a 4096 / fs),  T_lo[b] = exp(2 pi i b / fs)  (each in double, rounded to float),
+ *   out = v * conj(p):  pr = hi.re lo.re - hi.im lo.im, pi = hi.re lo.im + hi.im lo.re, out = (v.re pr + v.im pi, v.im pr - v.re pi),
+ * every product and sum rounded to float.  f = 0: out = v.  The engine computes the same bits on the GPU.  0, or AISGPU_EINVAL for an
+ * unknown format, sample_rate < 1, first_sample < 0, n < 0, null buffers, or an offset outside (-fs/2, fs/2). */
+int aisgpu_tune_restate(int format, int sample_rate, int32_t offset_hz, int64_t first_sample, const void *in, int64_t n, void *out_cf32);
 
 /* == AIS::Message::getBinaryNMEA(out, tag, crc) (Message.cpp:277-396): 0xAC 0x00 framed, byte-stuffed binary record with an
  * optional CRC-16 (Helper.cpp:42-57).  Returns the bytes written, 0 when the reference would emit nothing. Host-only. */
