@@ -21,6 +21,8 @@
  *   FM / PhaseSearch(EMA) ......... DSP/Demod.cpp:27-170, Demod.h:27-31
  *   rate -> chain table ........... DSP/Model.cpp:109-356
  *   ModelBase/Standard/Default .... DSP/Model.cpp:419-438, 484-577
+ *   ModelChallenger ............... DSP/Model.cpp:601-678
+ *   single-channel mode at 48k .... DSP/Model.cpp:35-107 (-c X: convert >> FCIC5_a)
  *   Decoder ....................... Marine/AIS.h:91-181, AIS.cpp:33-142
  *   Message bits + NMEA ........... Marine/Message.h:181-194,264-281, Message.cpp:28-39,398-413,569-686
  */
@@ -150,7 +152,10 @@ typedef struct Chan {
 	long long sample_idx;
 	PSEma ema[5];
 	PSearch ps[5];
-	Decoder dec[5];
+	Decoder dec[10]; /* ModelChallenger: 0..4 behind the coherent branch, 5..9 (FM phase d - 5) behind the FM branch */
+	/* ModelChallenger: the FM branch's Filter 37 outputs of the group of five in flight, and how far its order has stepped */
+	float fm_val[5];
+	int fm_n, grp_done, lvl_set;
 	/* SimplePLL */
 	int pll_prev;
 	float pll;
@@ -167,15 +172,20 @@ typedef struct {
 	cf *out; long outcap;
 } Stage;
 
-enum { MODEL_STANDARD = 0, MODEL_BASE = 1, MODEL_DEFAULT = 2 };
-enum { FLAG_PS_EMA = 1, FLAG_AFC_WIDE = 2, FLAG_DROOP = 4, FLAG_TAPS = 8 };
+enum { MODEL_STANDARD = 0, MODEL_BASE = 1, MODEL_DEFAULT = 2, MODEL_CHALLENGER = 4 };
+enum { FLAG_PS_EMA = 1, FLAG_AFC_WIDE = 2, FLAG_DROOP = 4, FLAG_TAPS = 8, FLAG_MODE_X = 64 };
+/* ModelChallenger's order of its ten decoders within a group of five samples (decoder d < 5: coherent phase d, d >= 5: FM phase
+ * d - 5): f0 f1 f2 f3 | a0 a1 a2 a3 a4 | f4 (see chall_sample) */
+static const int CHALLENGER_ORDER[10] = { 5, 6, 7, 8, 0, 1, 2, 3, 4, 9 };
 #define NTAPS_C 9
 #define NTAPS_F 14
 
 typedef struct Handle {
 	int model, sample_rate, format, own_mmsi;
 	unsigned flags;
-	int ps_ema, afc_wide, taps_on;
+	int ps_ema, afc_wide, taps_on, mode_x;
+	int order[10];
+	int *pub; long npub, pubcap; /* the decoder that published each message not yet read (Decoder.idx) */
 	Stage st[12];
 	int nst;
 	cf rot, mult;
@@ -288,7 +298,8 @@ static void dec_signal_out(Decoder *d, int sig) { /* DecoderMessage.Send: Model.
 		return;
 	}
 	if (sig != SIG_RESET) return; /* sibling decoders only act on Reset (AIS.cpp:98-108) */
-	for (int j = 0; j < 5; j++)
+	int n = h->model == MODEL_CHALLENGER ? 10 : 5; /* Model.cpp:654-673: all ten decoders of a channel are cross-connected */
+	for (int j = 0; j < n; j++)
 		if (j != d->idx) dec_next_state(&c->dec[j], S_TRAINING, 0);
 }
 
@@ -354,6 +365,11 @@ static int dec_process(Decoder *d, int len) { /* AIS.cpp:66-96 */
 			build_nmea(h, d->data, length, d->ch->name, &h->text);
 			sv_push(&h->text, "\n", 1);
 			h->msg_count++;
+			if (h->npub == h->pubcap) {
+				h->pubcap = h->pubcap ? 2 * h->pubcap : 256;
+				h->pub = (int *)realloc(h->pub, h->pubcap * sizeof(int));
+			}
+			h->pub[h->npub++] = d->idx;
 		}
 		return 1;
 	}
@@ -610,6 +626,69 @@ static float cgf_correct(Handle *h, Cgf *g) {
 	g->rot.im /= a;
 	return f * 48000.0f / 162.0f;
 }
+/* DSP::Filter (DSP.cpp:249-280) */
+static float firf_dot(const FirF *f, const float *d) {
+	float x = 0.0f;
+	for (int i = 0; i < f->nt; i++) x += f->taps[i] * d[i];
+	return x;
+}
+
+/* ModelChallenger (Model.cpp:601-678): the throttle (a one-way Deinterleave) hands each CGF output sample on alone, first to the
+ * coherent branch (FilterComplex 17 -> ScatterPLL -> PhaseSearchEMA nDelay 3), then to the FM branch (FM -> Filter 37 ->
+ * Deinterleave).  ScatterPLL hands a group of five out when its fifth sample arrives; Deinterleave hands FM phase j out at the
+ * group's sample j.  The ten decoders step in h->order within each group: a decoder steps as soon as its input exists and every
+ * decoder ahead of it in the order has stepped.  ScatterPLL writes the group's level into the tag just before the first coherent
+ * decoder steps, so with the reference's order f0..f3 read the previous group's level (or the other channel's, the TAG being
+ * shared) and f4 the current one. */
+static void chall_sample(Chan *c, cf x) {
+	Handle *h = c->h;
+	Tag *tag = &h->tag;
+	int taps = !h->mode_x; /* the single-channel harness records ModelChallenger's front-end taps only (ref_harness.cpp) */
+	FirC *fc = &c->fc;
+	for (int i = 1; i < fc->nt; i++) fc->buffer[i - 1] = fc->buffer[i]; /* DSP.cpp:219-225, len < ntaps */
+	fc->buffer[fc->nt - 1] = x;
+	cf y = firc_dot(fc, fc->buffer);
+	if (taps) tapc(h, 7 + c->id, &y, 1);
+	c->sample[c->lastSymbol++] = y;
+	if (tag->mode & 1) c->level += y.re * y.re + y.im * y.im;
+
+	cf cj = { c->fm_prev.re, -c->fm_prev.im }; /* Demod.cpp:27-37 */
+	cf p = cmul(x, cj);
+	float v = atan2f(p.im, p.re) / PI_F;
+	c->fm_prev = x;
+	if (taps) tapf(h, 10 + c->id, &v, 1);
+	FirF *fr = &c->fr;
+	for (int i = 1; i < fr->nt; i++) fr->buffer[i - 1] = fr->buffer[i]; /* DSP.cpp:253-259, len < ntaps */
+	fr->buffer[fr->nt - 1] = v;
+	v = firf_dot(fr, fr->buffer);
+	if (taps) tapf(h, 12 + c->id, &v, 1);
+	c->fm_val[c->fm_n++] = v;
+
+	while (c->grp_done < 10) {
+		int d = h->order[c->grp_done];
+		if (d < 5) {
+			if (c->lastSymbol < 5) break;
+			if (!c->lvl_set && (tag->mode & 1)) tag->sample_lvl = c->level / 5;
+			c->lvl_set = 1;
+			tag->sample_idx = c->sample_idx + d;
+			float b = psema_step(&c->ema[d], c->sample[d], 3);
+			if (taps) tapf(h, c->id * 5 + d, &b, 1);
+			dec_run(&c->dec[d], b);
+		}
+		else {
+			if (d - 5 >= c->fm_n) break;
+			tag->sample_idx = c->sample_idx + d - 5;
+			dec_run(&c->dec[d], c->fm_val[d - 5]);
+		}
+		c->grp_done++;
+	}
+	if (c->grp_done == 10) {
+		c->sample_idx += 5;
+		c->level = 0.0f;
+		c->lastSymbol = c->fm_n = c->grp_done = c->lvl_set = 0;
+	}
+}
+
 static void cgf_receive(Chan *c, const cf *data, int len) {
 	Handle *h = c->h;
 	Cgf *g = &c->cgf;
@@ -619,19 +698,15 @@ static void cgf_receive(Chan *c, const cf *data, int len) {
 		g->output[g->count] = data[i];
 		if (++g->count == 512) {
 			h->tag.ppm = cgf_correct(h, g);
-			tapc(h, 5 + c->id, g->output, 512);
-			firc_receive(c, &c->fc, g->output, 512, firout);
+			if (h->model != MODEL_CHALLENGER || !h->mode_x) tapc(h, 5 + c->id, g->output, 512);
+			if (h->model == MODEL_CHALLENGER)
+				for (int k = 0; k < 512; k++) chall_sample(c, g->output[k]);
+			else firc_receive(c, &c->fc, g->output, 512, firout);
 			g->count = 0;
 		}
 	}
 }
 
-/* DSP::Filter (DSP.cpp:249-280) */
-static float firf_dot(const FirF *f, const float *d) {
-	float x = 0.0f;
-	for (int i = 0; i < f->nt; i++) x += f->taps[i] * d[i];
-	return x;
-}
 
 /* Deinterleave (DSP.h:65-73) -> 5 decoders ; or SimplePLL (DSP.cpp:28-44) -> 1 decoder */
 static void fm_sink(Chan *c, const float *data, int len) {
@@ -700,7 +775,7 @@ static void fm_receive(Chan *c, const cf *data, int len) { /* Demod.cpp:27-37 */
 	firf_receive(c, &c->fr, out, len, h->tmpf2);
 }
 
-/* per-channel: Downsample2CIC5 (96k->48k) -> FilterCIC5 -> model back end (Model.cpp:341-346) */
+/* per-channel: [Downsample2CIC5 (96k->48k)] -> FilterCIC5 -> model back end (Model.cpp:341-346; single channel at 48k: 95-96) */
 static void chan_receive(Chan *c, const cf *data, int len) {
 	Handle *h = c->h;
 	if (h->tmpccap < len) {
@@ -710,14 +785,19 @@ static void chan_receive(Chan *c, const cf *data, int len) {
 	cf *y = h->tmpc, *o = h->tmpc + len;
 	int n = 0;
 	cf *s = c->ds2;
-	for (int i = 0; i < len; i += 2, n++) { /* DSP.cpp:93-117 */
-		cf z = data[i], r[5];
-		for (int k = 0; k < 5; k++) { r[k] = z; z.re += s[k].re; z.im += s[k].im; }
-		y[n].re = z.re * 0.03125f;
-		y[n].im = z.im * 0.03125f;
-		z = data[i + 1];
-		for (int k = 0; k < 5; k++) { s[k] = z; z.re += r[k].re; z.im += r[k].im; }
+	if (h->mode_x) {
+		memcpy(y, data, len * sizeof(cf));
+		n = len;
 	}
+	else
+		for (int i = 0; i < len; i += 2, n++) { /* DSP.cpp:93-117 */
+			cf z = data[i], r[5];
+			for (int k = 0; k < 5; k++) { r[k] = z; z.re += s[k].re; z.im += s[k].im; }
+			y[n].re = z.re * 0.03125f;
+			y[n].im = z.im * 0.03125f;
+			z = data[i + 1];
+			for (int k = 0; k < 5; k++) { s[k] = z; z.re += r[k].re; z.im += r[k].im; }
+		}
 	s = c->cic;
 	for (int i = 0; i < n; i += 2) { /* DSP.cpp:132-157 */
 		cf z = y[i], r[5];
@@ -730,7 +810,7 @@ static void chan_receive(Chan *c, const cf *data, int len) {
 		o[i + 1].im = z.im * 0.03125f;
 	}
 	tapc(h, 3 + c->id, o, n);
-	if (h->model == MODEL_DEFAULT) cgf_receive(c, o, n);
+	if (h->model == MODEL_DEFAULT || h->model == MODEL_CHALLENGER) cgf_receive(c, o, n);
 	else fm_receive(c, o, n);
 }
 
@@ -769,6 +849,11 @@ static void stage_out_reserve(Stage *s, long n) {
 }
 
 static void fe_run(Handle *h, int si, const cf *data, int len) {
+	if (h->mode_x) { /* convert >> FCIC5_a: channel A's chain alone */
+		tapc(h, 0, data, len);
+		chan_receive(&h->ch[0], data, len);
+		return;
+	}
 	if (si == h->nst) {
 		rot_receive(h, data, len);
 		return;
@@ -909,8 +994,10 @@ static int build_frontend(Handle *h) {
 
 /* ================= C entry points ================= */
 void *aisorc_create(int model, int sample_rate, int format, unsigned flags, int own_mmsi) {
-	if (model < 0 || model > 2 || format < 0 || format > 3) return NULL;
+	if (model < 0 || (model > 2 && model != MODEL_CHALLENGER) || format < 0 || format > 3) return NULL;
 	if (flags & (16u | 32u)) return NULL; /* -go FP_DS / DSK: checked against the compiled reference (ref_harness.cpp) only */
+	/* single-channel mode: ModelChallenger at 48k only (no US / DS2 in front), the one case pinned against the reference */
+	if ((flags & FLAG_MODE_X) && (sample_rate != 48000 || model != MODEL_CHALLENGER)) return NULL;
 	Handle *h = (Handle *)calloc(1, sizeof(Handle));
 	h->model = model;
 	h->sample_rate = sample_rate;
@@ -920,7 +1007,9 @@ void *aisorc_create(int model, int sample_rate, int format, unsigned flags, int 
 	h->ps_ema = (flags & FLAG_PS_EMA) != 0;
 	h->afc_wide = (flags & FLAG_AFC_WIDE) != 0;
 	h->taps_on = (flags & FLAG_TAPS) != 0;
-	if (build_frontend(h)) {
+	h->mode_x = (flags & FLAG_MODE_X) != 0;
+	memcpy(h->order, CHALLENGER_ORDER, sizeof(h->order));
+	if (!h->mode_x && build_frontend(h)) {
 		free(h);
 		return NULL;
 	}
@@ -933,7 +1022,7 @@ void *aisorc_create(int model, int sample_rate, int format, unsigned flags, int 
 		Chan *ch = &h->ch[c];
 		ch->h = h;
 		ch->id = c;
-		ch->name = c ? 'B' : 'A';
+		ch->name = h->mode_x ? 'X' : c ? 'B' : 'A';
 		ch->cgf.rot.re = 1.0f;
 		ch->fc.taps = (float *)TAPS_COHERENT;
 		ch->fc.nt = 17;
@@ -942,7 +1031,7 @@ void *aisorc_create(int model, int sample_rate, int format, unsigned flags, int 
 		ch->fr.nt = 37;
 		ch->fr.buffer = (float *)calloc(74, sizeof(float));
 		ch->pll_fast = 1;
-		for (int i = 0; i < 5; i++) {
+		for (int i = 0; i < 10; i++) {
 			ch->dec[i].ch = ch;
 			ch->dec[i].idx = i;
 			ch->dec[i].state = S_TRAINING;
@@ -1014,6 +1103,33 @@ long aisorc_tap_f(void *hv, int tap, float *dst, long max) {
 	return take(&((Handle *)hv)->tf[tap], dst, max);
 }
 long aisorc_msg_count(void *hv) { return ((Handle *)hv)->msg_count; }
+
+/* The decoder that published each message aisorc_messages has not yet returned, in the same order (Decoder.idx: the phase for
+ * models 0 and 2, 0 for model 1; for ModelChallenger 0..4 the coherent phases, 5..9 the FM phases).  Copies up to max and clears
+ * when dst != NULL; returns the count. */
+long aisorc_publishers(void *hv, int *dst, long max) {
+	Handle *h = (Handle *)hv;
+	long n = h->npub;
+	if (dst) {
+		long k = n < max ? n : max;
+		memcpy(dst, h->pub, k * sizeof(int));
+		h->npub = 0;
+	}
+	return n;
+}
+
+/* Test hook: ModelChallenger's order of its ten decoders within a group (numbered as by aisorc_publishers).  The reference's is
+ * CHALLENGER_ORDER; any permutation is accepted, anything else refused (-1). */
+int aisorc_challenger_order(void *hv, const int order[10]) {
+	Handle *h = (Handle *)hv;
+	int seen = 0;
+	for (int i = 0; i < 10; i++) {
+		if (order[i] < 0 || order[i] > 9 || (seen >> order[i] & 1)) return -1;
+		seen |= 1 << order[i];
+	}
+	memcpy(h->order, order, sizeof(h->order));
+	return 0;
+}
 long aisorc_messages(void *hv, char *dst, long max) {
 	Handle *h = (Handle *)hv;
 	long n = h->text.n;
@@ -1047,5 +1163,6 @@ void aisorc_destroy(void *hv) {
 	free(h->tmpf2);
 	free(h->tmpc);
 	free(h->text.p);
+	free(h->pub);
 	free(h);
 }

@@ -26,6 +26,8 @@ long aisorc_tap_ppm(void *h, int tap, float *dst, long max);
 long aisorc_tap_f(void *h, int tap, float *dst, long max);
 long aisorc_msg_count(void *h);
 long aisorc_messages(void *h, char *dst, long max);
+long aisorc_publishers(void *h, int *dst, long max);
+int aisorc_challenger_order(void *h, const int order[10]);
 void aisorc_destroy(void *h);
 
 #ifdef __cplusplus

@@ -2,7 +2,8 @@
 
 * ``RefModel``  : the UNMODIFIED reference (oracle/_ref/libaisref*.so, built by oracle/Makefile
                   from /root/reference where it lies; see ref_harness.cpp).
-* ``PortModel`` : the plain-C restatement (oracle/libaisoracle.so, ais_oracle.c).
+* ``PortModel`` : the plain-C restatement (oracle/libaisoracle.so, ais_oracle.c): models 0, 1, 2 and 4 (ModelChallenger), and
+                  ModelChallenger in single-channel mode at 48 kS/s (FLAG_MODE_X).
 
 Both expose the same methods so tests can swap them.  Only tests/, __graft_entry__.smoke() and
 bench.py's cpu_baseline / --impl reference legs may import this module; the product never does.
@@ -13,9 +14,13 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
-MODEL_STANDARD, MODEL_BASE, MODEL_DEFAULT, MODEL_CHALLENGER, MODEL_V2 = 0, 1, 2, 4, 11  # CHALLENGER / V2: reference harness only
+MODEL_STANDARD, MODEL_BASE, MODEL_DEFAULT, MODEL_CHALLENGER, MODEL_V2 = 0, 1, 2, 4, 11  # V2: reference harness only
 FMT_CF32, FMT_CU8, FMT_CS8, FMT_CS16 = 0, 1, 2, 3
 FLAG_PS_EMA, FLAG_AFC_WIDE, FLAG_DROOP, FLAG_TAPS, FLAG_FP_DS, FLAG_DSK = 1, 2, 4, 8, 16, 32  # FP_DS / DSK: reference harness only
+FLAG_MODE_X = 64  # the port only: single-channel mode (-c X), ModelChallenger at 48 kS/s; the reference's is oracle_x.RefModelX
+# ModelChallenger's decoders as publishers() numbers them: 0..4 the coherent phases a0..a4, 5..9 the FM phases f0..f4.  The
+# reference steps them in this order within each group of five 48 kHz samples (PortModel.challenger_order replaces it).
+CHALLENGER_ORDER = (5, 6, 7, 8, 0, 1, 2, 3, 4, 9)
 DEFAULT_FLAGS = FLAG_PS_EMA | FLAG_AFC_WIDE | FLAG_DROOP
 
 # complex taps
@@ -81,6 +86,10 @@ def _bind(lib, prefix):
     f = getattr(lib, prefix + "_destroy")
     f.restype = None
     f.argtypes = [C.c_void_p]
+    f = getattr(lib, prefix + "_publishers", None)
+    if f is not None:
+        f.restype = C.c_long
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_long]
 
 
 _libs = {}
@@ -172,6 +181,16 @@ class _Model:
         txt = buf.raw[:n].decode("ascii", "replace")
         return [Msg(l) for l in txt.split("\n") if l]
 
+    def publishers(self):
+        """The decoder that published each message messages() has not yet returned, in order (see CHALLENGER_ORDER for
+        ModelChallenger's numbering; the reference harness records ModelChallenger's only).  Call it before messages()."""
+        f = getattr(self.lib, self.p + "_publishers")
+        n = f(self.h, None, 0)
+        out = np.zeros(n, dtype=np.int32)
+        if n:
+            f(self.h, out.ctypes.data_as(C.c_void_p), n)
+        return out.tolist()
+
     def close(self):
         if self.h:
             getattr(self.lib, self.p + "_destroy")(self.h)
@@ -196,3 +215,12 @@ class PortModel(_Model):
 
     def __init__(self, *a, **kw):
         super().__init__(_load(port_lib_path(), "aisorc"), *a, **kw)
+
+    def challenger_order(self, order):
+        """Test hook: step ModelChallenger's ten decoders in this order (a permutation of 0..9) within each group."""
+        f = self.lib.aisorc_challenger_order
+        f.restype = C.c_int
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        a = (C.c_int * 10)(*order)
+        if f(self.h, a) != 0:
+            raise ValueError("not a permutation of the ten decoders: %r" % (order,))

@@ -7,7 +7,8 @@
 // feeds them RAW blocks of a caller-chosen chunk length through a
 // Device::Device subclass (Source/Device/Device.h:58) exactly as a device thread
 // would (Source/Device/FileRAW.cpp:121-137), and records
-//   * every AIS::Message the model publishes (Source/DSP/Model.h:87,96), and
+//   * every AIS::Message the model publishes (Source/DSP/Model.h:87,96), for ModelChallenger with the
+//     decoder that published it (aisref_publishers), and
 //   * optional float taps on the internal Connection<>s of the chain
 // so that the CPU restatement in oracle/ais_oracle.c and the CUDA path can be
 // compared against the real thing.  Built with -fno-access-control so private
@@ -104,6 +105,16 @@ struct MsgSink : public StreamIn<AIS::Message> {
 	}
 };
 
+// Which decoder published: one more sink on each decoder's own output, behind the model's output (so it hears each message
+// right after MsgSink has recorded it).  code numbers the decoder as ais_oracle.c's Decoder.idx does.
+struct PubSink : public StreamIn<AIS::Message> {
+	std::vector<int> *dst = nullptr;
+	int code = 0;
+	void Receive(const AIS::Message *, int len, TAG &) {
+		for (int i = 0; i < len; i++) dst->push_back(code);
+	}
+};
+
 enum { MODEL_STANDARD = 0, MODEL_BASE = 1, MODEL_DEFAULT = 2, MODEL_CHALLENGER = 4, MODEL_V2 = 11 };
 enum { FLAG_PS_EMA = 1, FLAG_AFC_WIDE = 2, FLAG_DROOP = 4, FLAG_TAPS = 8, FLAG_FP_DS = 16, FLAG_DSK = 32 };
 static const int NTAPS_C = 11; // 0: ROT in, 1/2: ROT up/down, 3/4: C_a/C_b, 5/6: CGF or (unused), 7/8: FC, 9: US out, 10: DSK out
@@ -119,6 +130,8 @@ struct Handle {
 	bool taps = false;
 	AIS::ModelFrontend *fe = nullptr;
 	MsgSink sink;
+	PubSink pub[2][10];
+	std::vector<int> pubs;
 	RecC tc[NTAPS_C];
 	RecF tf[NTAPS_F];
 	Format fmt = Format::CF32;
@@ -130,6 +143,34 @@ struct Handle {
 		delete mc;
 	}
 };
+
+// ModelChallenger: the publisher sinks on DEC_a / DEC_af (codes 0..4 / 5..9) and DEC_b / DEC_bf, and in A/B mode its taps
+// (complex 5/6: CGF, 7/8: FC; float 0..4 / 5..9: CD_EMA per phase, 10/11: FM, 12/13: FR).  In single-channel mode its taps stay
+// the front end's, as tests/golden/mode_x.json records them.
+static void attach_challenger(Handle *h, bool two_channels) {
+	AIS::ModelChallenger *m = h->mc;
+	for (int c = 0; c < (two_channels ? 2 : 1); c++)
+		for (int i = 0; i < 5; i++) {
+			for (int k = 0; k < 2; k++) {
+				PubSink &ps = h->pub[c][5 * k + i];
+				ps.dst = &h->pubs;
+				ps.code = 5 * k + i;
+				AIS::Decoder &d = c ? (k ? m->DEC_bf[i] : m->DEC_b[i]) : (k ? m->DEC_af[i] : m->DEC_a[i]);
+				d.out.Connect(&ps);
+			}
+		}
+	if (!h->taps || !two_channels) return;
+	m->CGF_a.out.Connect(&h->tc[5]);
+	m->FC_a.out.Connect(&h->tc[7]);
+	m->FM_af.out.Connect(&h->tf[10]);
+	m->FR_af.out.Connect(&h->tf[12]);
+	for (int i = 0; i < 5; i++) m->CD_EMA_a[i].out.Connect(&h->tf[i]);
+	m->CGF_b.out.Connect(&h->tc[6]);
+	m->FC_b.out.Connect(&h->tc[8]);
+	m->FM_bf.out.Connect(&h->tf[11]);
+	m->FR_bf.out.Connect(&h->tf[13]);
+	for (int i = 0; i < 5; i++) m->CD_EMA_b[i].out.Connect(&h->tf[5 + i]);
+}
 
 template <typename T>
 bool feeds(Connection<T> &c, StreamIn<T> *s) {
@@ -240,6 +281,7 @@ void *aisref_create(int model, int sample_rate, int format, unsigned flags, int 
 				h->mb->sampler_b.out.Connect(&h->tf[5]);
 			}
 		}
+		if (h->mc) attach_challenger(h, true);
 	}
 	catch (const std::exception &e) {
 		fprintf(stderr, "aisref_create: %s\n", e.what());
@@ -314,6 +356,19 @@ long aisref_tap_f(void *hv, int tap, float *dst, long max) {
 }
 
 long aisref_msg_count(void *hv) { return ((Handle *)hv)->sink.count; }
+
+// ModelChallenger: the decoder that published each message aisref_messages has not yet returned, in the same order (0..4 the
+// coherent phases, 5..9 the FM phases).  Copies up to max and clears when dst != NULL; returns the count.
+long aisref_publishers(void *hv, int *dst, long max) {
+	std::vector<int> &v = ((Handle *)hv)->pubs;
+	long n = (long)v.size();
+	if (dst) {
+		long k = n < max ? n : max;
+		memcpy(dst, v.data(), k * sizeof(int));
+		v.clear();
+	}
+	return n;
+}
 
 // newline-separated records "ch|nbits|start_idx|end_idx|level|ppm|HEXPAYLOAD|nmea1 nmea2"
 long aisref_messages(void *hv, char *dst, long max) {

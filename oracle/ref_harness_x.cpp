@@ -73,6 +73,7 @@ extern "C" void *aisrefx_create(int model, int sample_rate, int format, unsigned
 				h->mb->sampler_a.out.Connect(&h->tf[0]);
 			}
 		}
+		if (h->mc) attach_challenger(h, false);
 	}
 	catch (const std::exception &e) {
 		fprintf(stderr, "aisrefx_create: %s\n", e.what());

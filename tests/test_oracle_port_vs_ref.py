@@ -15,6 +15,7 @@ import pytest
 import aissynth as S
 import golden_util as G
 import oracle as O
+import oracle_x as OX
 
 STORE = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "port_vs_ref.json")
 CASES = []  # (case id, compare() arguments), filled below by case()
@@ -25,12 +26,22 @@ def case(name, model, fs, N, nchunks, **kw):
     return name
 
 
-def digest(Model, model, fs, N, nchunks, fmt=O.FMT_CF32, flags=O.DEFAULT_FLAGS, seed=0, multi=False, schedule=None):
+def digest(Model, model, fs, N, nchunks, fmt=O.FMT_CF32, flags=O.DEFAULT_FLAGS, seed=0, multi=False, schedule=None, x_mode=False):
     """Runs one model over the seeded stimulus; returns the input hash, one hash over every tap of every chunk (in order,
-    with lengths) and the per-chunk message records.  schedule: the length of every chunk (instead of nchunks chunks of N)."""
+    with lengths) and the per-chunk message records.  schedule: the length of every chunk (instead of nchunks chunks of N).
+    x_mode: single-channel mode (the reference's oracle_x.RefModelX) on mode_x_util's stimulus at 0 Hz.  For ModelChallenger
+    the records also name the decoder that published each message."""
     lengths = list(schedule) if schedule is not None else [N] * nchunks
     offs = np.cumsum([0] + lengths)
-    x = S.random_stream(fs, int(offs[-1]), seed, multi_sentence=multi)[0]
+    if x_mode:
+        import mode_x_util as MX
+        x = MX.x_stream(fs, int(offs[-1]), seed)[0]
+        if Model is O.RefModel:
+            Model = OX.RefModelX
+        else:
+            flags |= O.FLAG_MODE_X
+    else:
+        x = S.random_stream(fs, int(offs[-1]), seed, multi_sentence=multi)[0]
     per = 1
     if fmt == O.FMT_CU8:
         x, per = S.to_cu8(x), 2
@@ -51,7 +62,9 @@ def digest(Model, model, fs, N, nchunks, fmt=O.FMT_CF32, flags=O.DEFAULT_FLAGS, 
             a = np.ascontiguousarray(a)
             h.update(np.int64(a.size).tobytes())
             h.update(a.tobytes())
-        msgs.append([G.msg_record(q.channel, q.nbits, q.payload, q.nmea, q.start_idx, q.end_idx, q.level, q.ppm) for q in m.messages()])
+        pubs = m.publishers() if model == O.MODEL_CHALLENGER else None
+        recs = [G.msg_record(q.channel, q.nbits, q.payload, q.nmea, q.start_idx, q.end_idx, q.level, q.ppm) for q in m.messages()]
+        msgs.append(recs if pubs is None else [[r, p] for r, p in zip(recs, pubs)])
     return {"input_sha256": hashlib.sha256(np.ascontiguousarray(x).tobytes()).hexdigest(), "taps_sha256": h.hexdigest(), "messages": msgs}
 
 
@@ -69,7 +82,7 @@ def compare(name):
     for c, (g, w) in enumerate(zip(got["messages"], want["messages"])):
         assert g == w, "messages differ in chunk %d" % c
     assert got == want, "taps differ from the reference's"
-    if O.have_ref():
+    if O.have_ref() and (not kw.get("x_mode") or OX.have_refx()):
         assert digest(O.RefModel, *args, **kw) == want, "the reference no longer reproduces tests/golden/port_vs_ref.json"
     return sum(len(c) for c in want["messages"])
 
@@ -90,6 +103,14 @@ SCHED_RATES = {1536000: 64, 96000: 4, 6144000: 256}
 SCHEDULES = {(m, fs, f): case("schedule_m%d_%d_f%d" % (m, fs, f), m, fs, 0, 0, fmt=f, seed=61, schedule=[g * u for u in SCHEDULE])
              for m in (O.MODEL_DEFAULT, O.MODEL_STANDARD, O.MODEL_BASE) for fs, g in SCHED_RATES.items()
              for f in ((O.FMT_CF32, O.FMT_CU8) if fs == 1536000 else (O.FMT_CF32,))}
+# ModelChallenger: its ten decoders (with the publisher of every message), its CGF / FIR17 / FM / Filter 37 taps and the coherent
+# decoders' inputs; AB at 96 and 1536 kS/s, AFC_WIDE on and off, a changing submit schedule, and single-channel mode at 48 kS/s
+CHALLENGER = {"96k": case("challenger_96k", O.MODEL_CHALLENGER, 96000, 4096, 24, seed=41),
+              "1536k": case("challenger_1536k", O.MODEL_CHALLENGER, 1536000, 65536, 4, seed=43),
+              "96k_afc_narrow": case("challenger_96k_afc_narrow", O.MODEL_CHALLENGER, 96000, 4096, 24, flags=O.FLAG_PS_EMA | O.FLAG_DROOP,
+                                     seed=47),
+              "schedule_96k": case("challenger_schedule_96k", O.MODEL_CHALLENGER, 96000, 0, 0, seed=61, schedule=[4 * u for u in SCHEDULE]),
+              "x_48k": case("challenger_x_48k", O.MODEL_CHALLENGER, 48000, 2048, 24, seed=53, x_mode=True)}
 
 
 @pytest.mark.parametrize("model", [O.MODEL_DEFAULT, O.MODEL_STANDARD, O.MODEL_BASE])
@@ -133,9 +154,16 @@ def test_changing_chunk_lengths(built, key):
     assert compare(SCHEDULES[key]) >= 1
 
 
-if __name__ == "__main__":  # regenerate the stored outputs from the reference (needs oracle/_ref)
-    assert O.have_ref(), "oracle/_ref/libaisref.so not built"
-    out = {name: digest(O.RefModel, *args, **kw) for name, args, kw in CASES}
+@pytest.mark.parametrize("key", sorted(CHALLENGER))
+def test_challenger(built, key):
+    assert compare(CHALLENGER[key]) >= 2
+
+
+if __name__ == "__main__":  # regenerate the stored outputs from the reference (needs oracle/_ref): all cases, or those named
+    import sys
+    assert O.have_ref() and OX.have_refx(), "oracle/_ref not built"
+    out = load_store()
+    out.update({name: digest(O.RefModel, *args, **kw) for name, args, kw in CASES if len(sys.argv) < 2 or name in sys.argv[1:]})
     with open(STORE, "w") as f:
         json.dump(out, f, indent=0, sort_keys=True)
         f.write("\n")
