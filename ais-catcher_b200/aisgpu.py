@@ -27,7 +27,8 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_check_attach", "aisgpu_dump_open", "aisgpu_dump_close", "aisgpu_wav_probe", "aisgpu_feed_wav_files",
            "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json", "aisgpu_msg_format", "aisgpu_lines_enable",
            "aisgpu_poll_lines", "aisgpu_set_receivers", "aisgpu_check_receivers",
-           "aisgpu_set_tuning", "aisgpu_check_tuning", "aisgpu_tune_restate"]
+           "aisgpu_set_tuning", "aisgpu_check_tuning", "aisgpu_tune_restate", "aisgpu_set_clock", "aisgpu_check_clock",
+           "aisgpu_stamp"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 # message formats: positions in the reference's enum class MessageFormat (MSGFORMAT of its outputs); include/aisgpu.h describes each record
@@ -101,6 +102,22 @@ def check_tuning(offsets, **engine):
     Raises with the reason if the offsets (Hz, one per stream) would be refused."""
     lib = load()
     rc = lib.aisgpu_check_tuning(C.byref(make_config(**engine)), _offsets(offsets), len(offsets))
+    if rc:
+        raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode("latin-1")))
+
+
+def _starts(start_us):
+    return None if start_us is None else (C.c_int64 * max(len(start_us), 1))(*[int(t) for t in start_us])
+
+
+def check_clock(start_us, n=None, **engine):
+    """aisgpu_check_clock (no GPU needed): the rules of Engine.set_clock for an engine of keyword arguments `engine`.  start_us: one
+    start time (microseconds since the epoch) per stream, or None for the live clock; n: the count passed (default: len(start_us),
+    or n_streams for None).  Raises with the reason if the clock would be refused."""
+    lib = load()
+    if n is None:
+        n = engine.get("n_streams", 1) if start_us is None else len(start_us)
+    rc = lib.aisgpu_check_clock(C.byref(make_config(**engine)), _starts(start_us), int(n))
     if rc:
         raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode("latin-1")))
 
@@ -211,6 +228,10 @@ def load():
         lib.aisgpu_set_tuning.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
         lib.aisgpu_check_tuning.argtypes = [C.POINTER(Config), C.POINTER(C.c_int32), C.c_int]
         lib.aisgpu_tune_restate.argtypes = [C.c_int, C.c_int, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+    if hasattr(lib, "aisgpu_set_clock"):  # absent from libraries built before the clocks (AISGPU_LIB)
+        lib.aisgpu_set_clock.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int]
+        lib.aisgpu_check_clock.argtypes = [C.POINTER(Config), C.POINTER(C.c_int64), C.c_int]
+        lib.aisgpu_stamp.argtypes = [C.c_void_p, C.c_int, C.c_int64, C.POINTER(C.c_int64)]
     lib.aisgpu_validate.argtypes = [C.c_char_p, C.c_int]
     lib.aisgpu_build_nmea.argtypes = [C.POINTER(MsgStruct), C.c_int, C.POINTER(C.c_int)]
     lib.aisgpu_msg_json.argtypes = [C.POINTER(MsgStruct), C.POINTER(TagStruct), C.c_char_p, C.c_int]
@@ -560,6 +581,18 @@ class Engine:
         """aisgpu_set_tuning: one offset in Hz per stream (the channel pair's centre, or in X mode the channel, relative to the
         capture's centre), before the first submit and at most once.  Each submit is then mixed on the GPU so that it lands at 0 Hz."""
         self._chk(self.lib.aisgpu_set_tuning(self.h, _offsets(offsets), len(offsets)))
+
+    def set_clock(self, start_us=None):
+        """aisgpu_set_clock: start_us, one start time per stream in microseconds since the epoch (a recording clock), or None (the
+        live clock), before the first submit and at most once.  Every record then carries its frame's own receive time."""
+        n = self.n_streams if start_us is None else len(start_us)
+        self._chk(self.lib.aisgpu_set_clock(self.h, _starts(start_us), n))
+
+    def stamp(self, stream, chunk):
+        """aisgpu_stamp: the receive time (microseconds since the epoch) of the frames of `stream` completed by submit `chunk`."""
+        t = C.c_int64(0)
+        self._chk(self.lib.aisgpu_stamp(self.h, int(stream), int(chunk), C.byref(t)))
+        return t.value
 
     def poll_lines(self, ticket=None, cap=1 << 20):
         """aisgpu_poll_lines: (bytes, number of records) of the frames of the submits up to ticket (None: all), in frame order."""

@@ -14,7 +14,9 @@
 #include <string.h>
 
 #include <algorithm>
+#include <chrono>
 #include <deque>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -114,6 +116,22 @@ struct Receiver {
 	int32_t driver = 0;
 	std::string hardware;
 	uint32_t ipv4 = 0;
+};
+
+// The receive time of every submit (aisgpu_set_clock), one per group: the leader's submits append to it and the members read it.
+// at[c] is S_c, the samples per stream submitted through submit c (counters[2] after it), for a recording clock, and the system
+// clock in microseconds since the epoch, read by submit c, for a live one.
+struct Clock {
+	bool live = false;
+	long long fs = 0;
+	std::vector<long long> start_us; // recording: the time of each stream's first sample
+	std::vector<long long> at;
+	// start_us[s] + floor(S_c * 10^6 / fs) without overflow, or the wall time of submit c
+	long long stamp(int s, long long c) const {
+		if (live) return at[(size_t)c];
+		const long long S = at[(size_t)c], q = S / fs, r = S % fs;
+		return start_us[(size_t)s] + q * 1000000 + r * 1000000 / fs;
+	}
 };
 
 } // namespace
@@ -259,6 +277,7 @@ struct aisgpu_handle {
 	std::vector<FrameRec> h_ring;
 	std::vector<aisgpu_msg> out_queue;
 	size_t out_pos = 0;
+	std::shared_ptr<Clock> clock; // aisgpu_set_clock (a member: its leader's); null: every record takes the output's rxtime_us
 	std::vector<int> seq; // per-stream multi-sentence sequence id (Message.cpp:28-39 is process-global in the reference)
 	std::vector<Receiver> rx; // per stream: the config's fields, or the receiver aisgpu_set_receivers installed
 	bool rx_table = false;    // aisgpu_set_receivers has been called: the records take the receivers' TAG fields
@@ -334,6 +353,8 @@ struct aisgpu_handle {
 	char *d_jstrings = nullptr, *d_jslots = nullptr, *d_jtext = nullptr;
 	aisgpu_msg *d_jmsg = nullptr;
 	int *d_jlen = nullptr, *d_jseg = nullptr, *d_jkeep = nullptr, *pin_jkeep = nullptr;
+	long long *d_jstamp = nullptr;    // with a clock: the stamps of a batch's frames, beside d_jmsg
+	std::vector<long long> json_stamp;
 	long long *d_jpsum = nullptr, *d_joff = nullptr, *d_jtotal = nullptr, *pin_jtotal = nullptr, *d_jgroups = nullptr;
 	char *pin_jtext = nullptr;
 	std::vector<int> json_seg;
@@ -1482,6 +1503,10 @@ int tune_input(aisgpu_handle *h, const void *&dev_in, long long &stride, int N) 
 // The caller's Receive(): N samples per stream in the caller's format.
 int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) {
 	if (int rc = check_outer(h, N)) return rc;
+	// Message::Stamp's reading of the system clock, once for every frame this submit completes
+	const long long wall_us = h->clock && h->clock->live ? (long long)std::chrono::duration_cast<std::chrono::microseconds>(
+															   std::chrono::system_clock::now().time_since_epoch()).count()
+														 : 0;
 	h->last_launches = 0;
 	if (h->tuned)
 		if (int rc = tune_input(h, dev_in, stride, N)) return rc;
@@ -1530,6 +1555,7 @@ int submit_outer(aisgpu_handle *h, const void *dev_in, long long stride, int N) 
 	}
 	h->counters[2] += (uint64_t)N;
 	h->counters[3] += 1;
+	if (h->clock) h->clock->at.push_back(h->clock->live ? wall_us : (long long)h->counters[2]);
 	return 0;
 }
 
@@ -1635,7 +1661,12 @@ int json_decode(aisgpu_handle *h, size_t q0) {
 		if (b0 == 0 || q[0].chunk != q[-1].chunk) carry = 0;
 		CU(cudaMemcpyAsync(h->d_jmsg, q, (size_t)n * sizeof(aisgpu_msg), cudaMemcpyHostToDevice, st));
 		CU(cudaMemcpyAsync(h->d_jseg, h->json_seg.data(), (size_t)n * sizeof(int), cudaMemcpyHostToDevice, st));
-		CU(fmt_launch(h->d_jmsg, n, h->d_fctx, h->rx_table, h->fmt_records, h->fmt_groups, h->d_jgroups, h->d_jslots, h->json_slot, h->rec_cap,
+		if (h->clock) { // each frame's stamp, from its stream and the submit that completed it
+			h->json_stamp.resize((size_t)n);
+			for (int i = 0; i < n; i++) h->json_stamp[i] = h->clock->stamp(q[i].stream, q[i].chunk);
+			CU(cudaMemcpyAsync(h->d_jstamp, h->json_stamp.data(), (size_t)n * sizeof(long long), cudaMemcpyHostToDevice, st));
+		}
+		CU(fmt_launch(h->d_jmsg, h->clock ? h->d_jstamp : nullptr, n, h->d_fctx, h->rx_table, h->fmt_records, h->fmt_groups, h->d_jgroups, h->d_jslots, h->json_slot, h->rec_cap,
 					  h->d_jlen, h->d_jseg, h->json_cap, carry, h->d_jpsum, h->d_joff, h->d_jkeep, h->d_jtotal, h->d_jtext, st));
 		CU(cudaMemcpyAsync(h->pin_jtotal, h->d_jtotal, 4 * sizeof(long long), cudaMemcpyDeviceToHost, st));
 		CU(cudaMemcpyAsync(h->pin_jkeep, h->d_jkeep, (size_t)n * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2206,7 +2237,7 @@ aisgpu_tag tag_of(const aisgpu_handle *h, int s) {
 int fmt_setup(aisgpu_handle *h) {
 	const int nctx = h->rx_table ? h->cfg.n_streams : 1;
 	std::vector<aisgpu_tag> tags((size_t)nctx);
-	std::vector<std::string> prefixes((size_t)nctx);
+	std::vector<AjPrefix> prefixes((size_t)nctx);
 	std::vector<size_t> hw_at((size_t)nctx), prefix_at((size_t)nctx);
 	std::string strings = h->fmt_uuid + '\0' + h->fmt_suffix + '\0';
 	size_t longest = 0, longest_prefix = 0;
@@ -2216,9 +2247,11 @@ int fmt_setup(aisgpu_handle *h) {
 		hw_at[i] = strings.size();
 		strings += std::string(tags[i].hardware) + '\0';
 		prefix_at[i] = strings.size();
-		strings += prefixes[i] + '\0';
-		longest = std::max(longest, prefixes[i].size() + strlen(tags[i].hardware) * 6);
-		longest_prefix = std::max(longest_prefix, prefixes[i].size());
+		strings += prefixes[i].text + '\0';
+		// the full-JSON line holds the prefix and, where the mode prints them, the time members of any stamp
+		const size_t line_head = prefixes[i].text.size() + ((tags[i].mode & 2) ? kAjTimeMax : 0);
+		longest = std::max(longest, line_head + strlen(tags[i].hardware) * 6);
+		longest_prefix = std::max(longest_prefix, line_head);
 	}
 	h->fmt_strings = strings;
 	// a record's room: the longest record of its format with the tag's strings (the hardware name escaped, uuid and suffix once per
@@ -2242,6 +2275,8 @@ int fmt_setup(aisgpu_handle *h) {
 		if (int rc = dalloc(h, &h->d_jpsum, kJsonBatch)) return rc;
 		if (int rc = dalloc(h, &h->d_joff, kJsonBatch)) return rc;
 	}
+	if (h->clock && !h->d_jstamp)
+		if (int rc = dalloc(h, &h->d_jstamp, kJsonBatch)) return rc;
 	dfree(h, h->d_jstrings);
 	dfree(h, h->d_fctx);
 	dfree(h, h->d_jslots);
@@ -2493,6 +2528,82 @@ int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) {
 	int sms = 0;
 	CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->cfg.device));
 	h->tune_ctas = 4 * sms;
+	return 0;
+}
+
+namespace {
+
+const long long kClockEnd = 253402300800000000LL; // 10000-01-01T00:00:00Z in microseconds: rxtime stays YYYYMMDDHHMMSS below it
+
+// The rules of aisgpu_set_clock that need no device: "" or the reason.
+std::string clock_refusal(const aisgpu_config &c, const int64_t *start_us, int n) {
+	if (n != c.n_streams) return "aisgpu_set_clock: " + std::to_string(n) + " start times for " + std::to_string(c.n_streams) + " streams";
+	if (start_us)
+		for (int s = 0; s < n; s++)
+			if (start_us[s] < 0 || start_us[s] >= kClockEnd)
+				return "aisgpu_set_clock: stream " + std::to_string(s) + ": start " + std::to_string((long long)start_us[s]) +
+					   " us must lie in [0, " + std::to_string(kClockEnd) + ") (1970-01-01 .. 9999-12-31)";
+	return "";
+}
+
+} // namespace
+
+int aisgpu_check_clock(const aisgpu_config *cfg, const int64_t *start_us, int n) {
+	aisgpu_config c;
+	if (!copy_config(cfg, &c)) {
+		g_create_error = "aisgpu_check_clock: null config or struct_size mismatch";
+		return AISGPU_EINVAL;
+	}
+	const std::string why = clock_refusal(c, start_us, n);
+	if (!why.empty()) {
+		g_create_error = why;
+		return AISGPU_EINVAL;
+	}
+	return 0;
+}
+
+int aisgpu_set_clock(aisgpu_handle *h, const int64_t *start_us, int n) {
+	ENTER(h);
+	std::string why = clock_refusal(h->given, start_us, n);
+	if (why.empty() && h->member)
+		why = "aisgpu_set_clock: this engine is a member of a group: its leader's clock stamps the group's frames (set it on the leader)";
+	if (why.empty() && h->clock) why = "aisgpu_set_clock: a clock is already set";
+	if (why.empty() && h->counters[3] > 0) why = "aisgpu_set_clock: the engine has been submitted to (set the clock before the first submit)";
+	if (!why.empty()) {
+		h->err = why;
+		return AISGPU_EINVAL;
+	}
+	auto clk = std::make_shared<Clock>();
+	clk->live = start_us == nullptr;
+	clk->fs = h->given.sample_rate;
+	if (start_us) clk->start_us.assign(start_us, start_us + n);
+	std::vector<aisgpu_handle *> group(1, h);
+	group.insert(group.end(), h->members.begin(), h->members.end());
+	for (aisgpu_handle *e : group) {
+		e->clock = clk;
+		if (e->json_on && !e->d_jstamp) { // a format enabled before the clock: the stamps' device buffer
+			if (int rc = dalloc(e, &e->d_jstamp, kJsonBatch)) return poison(h, rc);
+			CU(cudaStreamSynchronize(e->stream));
+		}
+	}
+	return 0;
+}
+
+int aisgpu_stamp(aisgpu_handle *h, int stream, int64_t chunk, int64_t *rxtime_us) {
+	if (!h || !rxtime_us) return AISGPU_EINVAL;
+	if (!h->clock) {
+		h->err = "aisgpu_stamp: the engine has no clock (aisgpu_set_clock)";
+		return AISGPU_EINVAL;
+	}
+	if (stream < 0 || stream >= h->cfg.n_streams) {
+		h->err = "aisgpu_stamp: no stream " + std::to_string(stream);
+		return AISGPU_EINVAL;
+	}
+	if (chunk < 0 || chunk >= (int64_t)h->clock->at.size()) {
+		h->err = "aisgpu_stamp: no submit " + std::to_string((long long)chunk) + " (" + std::to_string(h->clock->at.size()) + " so far)";
+		return AISGPU_EINVAL;
+	}
+	*rxtime_us = h->clock->stamp(stream, chunk);
 	return 0;
 }
 
@@ -2853,6 +2964,7 @@ int aisgpu_attach(aisgpu_handle *leader, const aisgpu_config *cfg, aisgpu_handle
 		return rc;
 	}
 	h->leader = leader;
+	h->clock = leader->clock; // a clock set before the attach (one set after it reaches the member through the leader)
 	leader->members.push_back(h);
 	*out = h;
 	return 0;

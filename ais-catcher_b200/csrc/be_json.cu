@@ -1455,8 +1455,8 @@ __host__ __device__ void usec(Out &o, long long t) {
 	else o.i64(t / 1000000);
 }
 
-// AIS::Message::getNMEAJSON (Message.cpp:93-191)
-__host__ __device__ void nmea_json(Out &o, const aisgpu_msg *m, const FmtCtx &c) {
+// AIS::Message::getNMEAJSON (Message.cpp:93-191); rxtime_us: the frame's stamp
+__host__ __device__ void nmea_json(Out &o, const aisgpu_msg *m, const FmtCtx &c, long long rxtime_us) {
 	o.cstr("{\"class\":\"AIS\",\"device\":\"AIS-catcher\",\"version\":");
 	o.i64(c.version);
 	o.cstr(",\"driver\":");
@@ -1479,7 +1479,7 @@ __host__ __device__ void nmea_json(Out &o, const aisgpu_msg *m, const FmtCtx &c)
 	}
 	if (c.mode & 2) {
 		o.cstr(",\"rxuxtime\":");
-		usec(o, c.rxtime_us);
+		usec(o, rxtime_us);
 	}
 	if (c.toa_us != 0) {
 		o.cstr(",\"toa\":");
@@ -1569,7 +1569,7 @@ __host__ __device__ void binary(Out &o, const char *start, const aisgpu_msg *m, 
 
 // AIS::Message::getNMEATagBlock (Message.cpp:198-285) with the engine's group counter: groups = the multi-sentence frames before
 // this one
-__host__ __device__ void tag_block(Out &o, const aisgpu_msg *m, const FmtCtx &c, long long groups) {
+__host__ __device__ void tag_block(Out &o, const aisgpu_msg *m, const FmtCtx &c, long long rxtime_us, long long groups) {
 	const int total = n_sent(m);
 	const int group = total > 1 ? (int)(groups % 9999) + 1 : 0;
 	for (int seq = 1; seq <= total; seq++) {
@@ -1578,7 +1578,7 @@ __host__ __device__ void tag_block(Out &o, const aisgpu_msg *m, const FmtCtx &c,
 		t.raw("s:s", 3);
 		t.i64(c.station);
 		t.raw(",c:", 3);
-		t.f64((double)c.rxtime_us / 1000000.0);
+		t.f64((double)rxtime_us / 1000000.0);
 		if (total > 1) {
 			t.raw(",g:", 3);
 			t.i64(seq);
@@ -1602,7 +1602,7 @@ __host__ __device__ void tag_block(Out &o, const aisgpu_msg *m, const FmtCtx &c,
 }
 
 // the screen's annotated sentences (OutputMessage::formatInto, MsgOut.h:73-106)
-__host__ __device__ void full_text(Out &o, const aisgpu_msg *m, const FmtCtx &c) {
+__host__ __device__ void full_text(Out &o, const aisgpu_msg *m, const FmtCtx &c, long long rxtime_us) {
 	for (int i = 0; i < n_sent(m); i++) {
 		o.raw(m->nmea[i], sent_len(m, i));
 		o.raw(" ( ", 3);
@@ -1623,7 +1623,7 @@ __host__ __device__ void full_text(Out &o, const aisgpu_msg *m, const FmtCtx &c)
 		}
 		if (c.mode & 2) {
 			o.cstr(", timestamp: ");
-			put_rxtime(o, c.rxtime_us);
+			put_rxtime(o, rxtime_us);
 		}
 		if (c.station) {
 			o.cstr(", ID: ");
@@ -1633,23 +1633,32 @@ __host__ __device__ void full_text(Out &o, const aisgpu_msg *m, const FmtCtx &c)
 	}
 }
 
-// one full-JSON line: prefix, body, '}'; its length, or -2 when it does not fit in cap
-__host__ __device__ int line(const aisgpu_msg *src, const char *prefix, int prefix_len, int mode, int station, char *out, int cap) {
+// one full-JSON line: the prefix with the time members of rxtime_us where the mode prints them (JSONAIS.cpp:1101-1106), body, '}';
+// its length, or -2 when it does not fit in cap
+__host__ __device__ int line(const aisgpu_msg *src, const FmtCtx &c, long long rxtime_us, char *out, int cap) {
 	Msg m;
 	for (int i = 0; i < kBufBytes; i++) m.d[i] = i < kMaxBytes ? src->data[i] : 0;
 	m.nbits = (src->nbits >= 0 && src->nbits <= kMaxBits) ? src->nbits : 0; // Message::setLength ignores other lengths
 	Out o(out, cap);
-	o.raw(prefix, prefix_len);
-	body(o, m, src, mode, station);
+	o.raw(c.prefix, c.prefix_time);
+	if (c.mode & 2) {
+		o.cstr(",\"rxtime\":\"");
+		put_rxtime(o, rxtime_us); // Message::getRxTime
+		o.cstr("\",\"rxuxtime\":");
+		o.f64((double)rxtime_us / 1000000.0);
+	}
+	o.raw(c.prefix + c.prefix_time, c.prefix_len - c.prefix_time);
+	body(o, m, src, c.mode, c.station);
 	o.ch('}');
 	return o.full ? -2 : (int)(o.p - out);
 }
 
 // The record of one frame in c.fmt (OutputMessage::formatInto, MsgOut.h:58-122, and OutputMessage::Receive for the JSON formats):
 // its length, or -2 when it does not fit in cap.  ordinal: the frames published before it; groups: the multi-sentence ones among
-// them.  JSON_SPARSE and JSON_ANNOTATED write the full line into scratch (scap bytes) first and rewrite it into out.
-__host__ __device__ int record(const aisgpu_msg *src, const FmtCtx &c, long long ordinal, long long groups, char *out, int cap,
-							   char *scratch, int scap) {
+// them; rxtime_us: its stamp.  JSON_SPARSE and JSON_ANNOTATED write the full line into scratch (scap bytes) first and rewrite it
+// into out.
+__host__ __device__ int record(const aisgpu_msg *src, const FmtCtx &c, long long rxtime_us, long long ordinal, long long groups, char *out,
+							   int cap, char *scratch, int scap) {
 	Out o(out, cap);
 	switch (c.fmt) {
 	case AISGPU_MSGFORMAT_NMEA:
@@ -1658,23 +1667,23 @@ __host__ __device__ int record(const aisgpu_msg *src, const FmtCtx &c, long long
 			o.cstr(c.suffix);
 		}
 		break;
-	case AISGPU_MSGFORMAT_NMEA_TAG: tag_block(o, src, c, groups); break;
+	case AISGPU_MSGFORMAT_NMEA_TAG: tag_block(o, src, c, rxtime_us, groups); break;
 	case AISGPU_MSGFORMAT_COMMUNITY_HUB:
-		if (ordinal % 100 == 0) nmea_json(o, src, c);
-		else binary(o, out, src, c.rxtime_us, false);
+		if (ordinal % 100 == 0) nmea_json(o, src, c, rxtime_us);
+		else binary(o, out, src, rxtime_us, false);
 		break;
-	case AISGPU_MSGFORMAT_BINARY_NMEA: binary(o, out, src, c.rxtime_us, c.crc != 0); break;
-	case AISGPU_MSGFORMAT_FULL: full_text(o, src, c); break;
-	case AISGPU_MSGFORMAT_JSON_NMEA: nmea_json(o, src, c); break;
+	case AISGPU_MSGFORMAT_BINARY_NMEA: binary(o, out, src, rxtime_us, c.crc != 0); break;
+	case AISGPU_MSGFORMAT_FULL: full_text(o, src, c, rxtime_us); break;
+	case AISGPU_MSGFORMAT_JSON_NMEA: nmea_json(o, src, c, rxtime_us); break;
 	case AISGPU_MSGFORMAT_JSON_FULL: {
-		const int n = line(src, c.prefix, c.prefix_len, c.mode, c.station, out, cap);
+		const int n = line(src, c, rxtime_us, out, cap);
 		if (n < 0) return -2;
 		o.p += n;
 		o.cstr(c.suffix);
 		break;
 	}
 	default: {
-		const int n = line(src, c.prefix, c.prefix_len, c.mode, c.station, scratch, scap);
+		const int n = line(src, c, rxtime_us, scratch, scap);
 		if (n < 0) return -2;
 		rewrite(o, scratch, n, c.fmt == AISGPU_MSGFORMAT_JSON_SPARSE ? D_SPARSE : D_ANNOTATED);
 		o.cstr(c.suffix);
@@ -1707,13 +1716,16 @@ __global__ void __launch_bounds__(256) k_fmt_groups(const aisgpu_msg *__restrict
 }
 
 // record i (frame ordinal + i) into the first cap bytes of its slot, the rest of the slot its scratch; its length into len[i].  The
-// context is ctx[0], or with per_stream that of the frame's stream (a receiver table)
-__global__ void k_fmt_records(const aisgpu_msg *__restrict__ msgs, int n, const FmtCtx *__restrict__ ctx, int per_stream, long long ordinal,
-							  const long long *__restrict__ groups, char *__restrict__ slots, int slot, int cap, int *__restrict__ len) {
+// context is ctx[0], or with per_stream that of the frame's stream (a receiver table); the time is stamps[i] (an engine with a
+// clock), else the context's
+__global__ void k_fmt_records(const aisgpu_msg *__restrict__ msgs, const long long *__restrict__ stamps, int n, const FmtCtx *__restrict__ ctx,
+							  int per_stream, long long ordinal, const long long *__restrict__ groups, char *__restrict__ slots, int slot, int cap,
+							  int *__restrict__ len) {
 	const int i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
 	char *s = slots + (size_t)i * slot;
-	len[i] = record(msgs + i, ctx[per_stream ? msgs[i].stream : 0], ordinal + i, groups[i], s, cap, s + cap, slot - cap);
+	const FmtCtx &c = ctx[per_stream ? msgs[i].stream : 0];
+	len[i] = record(msgs + i, c, stamps ? stamps[i] : c.rxtime_us, ordinal + i, groups[i], s, cap, s + cap, slot - cap);
 }
 
 // Where each record goes: record i is kept when the records of its submit up to and including it fit in cap bytes, and kept
@@ -1787,12 +1799,12 @@ __global__ void k_fmt_copy(const char *__restrict__ slots, int slot, const int *
 
 int fmt_record_host(const aisgpu_msg *m, const FmtCtx *c, long long ordinal, long long groups, char *out, int cap) {
 	const bool rewritten = c->fmt == AISGPU_MSGFORMAT_JSON_SPARSE || c->fmt == AISGPU_MSGFORMAT_JSON_ANNOTATED;
-	std::vector<char> scratch(rewritten ? (size_t)c->prefix_len + 4096 : 0);
-	const int n = record(m, *c, ordinal, groups, out, cap, scratch.data(), (int)scratch.size());
+	std::vector<char> scratch(rewritten ? (size_t)c->prefix_len + kAjTimeMax + 4096 : 0);
+	const int n = record(m, *c, c->rxtime_us, ordinal, groups, out, cap, scratch.data(), (int)scratch.size());
 	return n < 0 ? AISGPU_EOVERFLOW : n;
 }
 
-std::string aj_prefix(const aisgpu_tag *tag) {
+AjPrefix aj_prefix(const aisgpu_tag *tag) {
 	std::string s(256 + (tag->hardware ? strlen(tag->hardware) * 6 : 0), '\0');
 	Out o(&s[0], (int)s.size());
 	o.cstr("{\"class\":\"AIS\",\"device\":\"AIS-catcher\",\"version\":");
@@ -1801,34 +1813,29 @@ std::string aj_prefix(const aisgpu_tag *tag) {
 	o.i64(tag->driver);
 	o.cstr(",\"hardware\":");
 	o.qstr(tag->hardware ? tag->hardware : "");
-	if (tag->mode & 2) {
-		o.cstr(",\"rxtime\":\"");
-		put_rxtime(o, tag->rxtime_us); // Message::getRxTime
-		o.cstr("\",\"rxuxtime\":");
-		o.f64((double)tag->rxtime_us / 1000000.0);
-	}
+	const int time_at = (int)(o.p - &s[0]);
 	if (tag->toa_us) {
 		o.cstr(",\"toa\":");
 		o.f64((double)tag->toa_us / 1000000.0);
 	}
 	o.cstr(",\"scaled\":true");
 	s.resize((size_t)(o.p - &s[0]));
-	return s;
+	return AjPrefix{ s, time_at };
 }
 
-cudaError_t fmt_launch(const aisgpu_msg *d_msgs, int n, const FmtCtx *d_ctx, int per_stream, long long ordinal, long long groups, long long *d_groups,
+cudaError_t fmt_launch(const aisgpu_msg *d_msgs, const long long *d_stamps, int n, const FmtCtx *d_ctx, int per_stream, long long ordinal, long long groups, long long *d_groups,
 					   char *d_slots, int slot, int cap, int *d_len, const int *d_seg, long long budget, long long carry,
 					   long long *d_psum, long long *d_off, int *d_keep, long long *d_total, char *d_text, cudaStream_t st) {
 	if (n <= 0) return cudaSuccess;
 	k_fmt_groups<<<1, 256, 0, st>>>(d_msgs, n, groups, d_groups, d_total);
-	k_fmt_records<<<(n + 127) / 128, 128, 0, st>>>(d_msgs, n, d_ctx, per_stream, ordinal, d_groups, d_slots, slot, cap, d_len);
+	k_fmt_records<<<(n + 127) / 128, 128, 0, st>>>(d_msgs, d_stamps, n, d_ctx, per_stream, ordinal, d_groups, d_slots, slot, cap, d_len);
 	k_fmt_place<<<1, 256, 0, st>>>(d_len, d_seg, n, budget, carry, d_psum, d_off, d_keep, d_total);
 	k_fmt_copy<<<(n + 7) / 8, 256, 0, st>>>(d_slots, slot, d_keep, d_off, n, d_text);
 	return cudaGetLastError();
 }
 
 // the context of a tag: NULL strings as "" (suffix as given: NULL is none); prefix: aj_prefix(tag), which must outlive the context
-FmtCtx fmt_ctx(const aisgpu_tag *tag, int fmt, const char *suffix, const std::string &prefix) {
+FmtCtx fmt_ctx(const aisgpu_tag *tag, int fmt, const char *suffix, const AjPrefix &prefix) {
 	FmtCtx c;
 	c.fmt = fmt;
 	c.version = tag->version;
@@ -1844,14 +1851,15 @@ FmtCtx fmt_ctx(const aisgpu_tag *tag, int fmt, const char *suffix, const std::st
 	c.hardware = tag->hardware ? tag->hardware : "";
 	c.uuid = tag->uuid ? tag->uuid : "";
 	c.suffix = suffix ? suffix : "";
-	c.prefix = prefix.data();
-	c.prefix_len = (int)prefix.size();
+	c.prefix = prefix.text.data();
+	c.prefix_len = (int)prefix.text.size();
+	c.prefix_time = prefix.time_at;
 	return c;
 }
 
 extern "C" int aisgpu_msg_json_full(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int cap) {
 	if (!m || !tag || !out || cap <= 0) return AISGPU_EINVAL;
-	const std::string p = aj_prefix(tag);
+	const AjPrefix p = aj_prefix(tag);
 	const FmtCtx c = fmt_ctx(tag, AISGPU_MSGFORMAT_JSON_FULL, tag->suffix, p);
 	return fmt_record_host(m, &c, 0, 0, out, cap);
 }
@@ -1859,7 +1867,7 @@ extern "C" int aisgpu_msg_json_full(const aisgpu_msg *m, const aisgpu_tag *tag, 
 extern "C" int aisgpu_msg_format(const aisgpu_msg *m, const aisgpu_tag *tag, int msgformat, aisgpu_format_state *st, char *out, int cap) {
 	if (!m || !tag || !out || cap <= 0 || msgformat < AISGPU_MSGFORMAT_NMEA || msgformat > AISGPU_MSGFORMAT_JSON_ANNOTATED)
 		return AISGPU_EINVAL;
-	const std::string p = aj_prefix(tag);
+	const AjPrefix p = aj_prefix(tag);
 	const FmtCtx c = fmt_ctx(tag, msgformat, tag->suffix ? tag->suffix : "\r\n", p);
 	const int n = fmt_record_host(m, &c, st ? st->records : 0, st ? st->groups : 0, out, cap);
 	if (n >= 0 && st) {

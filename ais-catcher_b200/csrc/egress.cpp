@@ -17,14 +17,14 @@
 
 extern "C" int aisgpu_msg_json(const aisgpu_msg *m, const aisgpu_tag *tag, char *out, int cap) {
 	if (!m || !tag || !out || cap <= 0 || m->n_sentences < 0 || m->n_sentences > 4) return AISGPU_EINVAL;
-	const std::string no_prefix; // not printed by this format
+	const AjPrefix no_prefix; // not printed by this format
 	const FmtCtx c = fmt_ctx(tag, AISGPU_MSGFORMAT_JSON_NMEA, tag->suffix, no_prefix);
 	return fmt_record_host(m, &c, 0, 0, out, cap);
 }
 
 extern "C" int aisgpu_msg_binary(const aisgpu_msg *m, const aisgpu_tag *tag, int crc, uint8_t *out, int cap) {
 	if (!m || !tag || !out || cap <= 0) return AISGPU_EINVAL;
-	const std::string no_prefix; // not printed by this format
+	const AjPrefix no_prefix; // not printed by this format
 	FmtCtx c = fmt_ctx(tag, AISGPU_MSGFORMAT_BINARY_NMEA, nullptr, no_prefix);
 	c.crc = crc != 0;
 	return fmt_record_host(m, &c, 0, 0, (char *)out, cap);

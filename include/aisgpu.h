@@ -34,10 +34,9 @@ extern "C" {
 
 /* 3 since the engine groups; later additions are new entry points only (the full AIS JSON: aisgpu_msg_json_full, aisgpu_json_enable,
  * aisgpu_poll_json; the output records: aisgpu_msg_format, aisgpu_lines_enable, aisgpu_poll_lines; the receivers:
- * aisgpu_set_receivers, aisgpu_check_receivers; the tuning: aisgpu_set_tuning, aisgpu_check_tuning, aisgpu_tune_restate), so the
- * number callers check
- * against stays 3.  A caller that needs those entry points looks them up
- * (dlsym) instead of relying on the number. */
+ * aisgpu_set_receivers, aisgpu_check_receivers; the tuning: aisgpu_set_tuning, aisgpu_check_tuning, aisgpu_tune_restate; the
+ * receive time: aisgpu_set_clock, aisgpu_check_clock, aisgpu_stamp), so the number callers check against stays 3.  A caller that
+ * needs those entry points looks them up (dlsym) instead of relying on the number. */
 #define AISGPU_ABI_VERSION 3
 
 /* model kinds: the reference's "-m" numbers (Source/Application/Receiver.cpp:155-195) */
@@ -279,7 +278,8 @@ typedef struct aisgpu_tag {
 	int32_t mode;         /* TAG::mode: bit 0 -> signalpower/ppm are printed, bit 1 -> rxuxtime is printed */
 	int32_t status;       /* TAG::status, printed as msg_status when non-zero */
 	uint32_t ipv4;        /* TAG::ipv4, printed when non-zero */
-	int64_t rxtime_us;    /* Message::rxtime (microseconds since the epoch, Message::Stamp) */
+	int64_t rxtime_us;    /* Message::rxtime (microseconds since the epoch, Message::Stamp); an engine with a clock prints each frame's
+	                         stamp instead (aisgpu_set_clock) */
 	int64_t toa_us;       /* Message::toa, printed when non-zero */
 	int32_t station;      /* Message::getStation(), printed as station_id when non-zero */
 	int32_t include_ssl;  /* getNMEAJSON's include_ssl: print ssc (start_idx) and sl (end_idx - start_idx) */
@@ -404,7 +404,8 @@ int aisgpu_poll_lines(aisgpu_handle *h, int64_t ticket, char *out, size_t cap, s
  *     ends read a level switch per 48 kHz row;
  * -- and its records (aisgpu_poll_lines, aisgpu_poll_json) are printed with the output's tag whose station, driver, hardware, mode
  * (= tag_mode) and ipv4 are r[s]'s (Message::setOrigin, Message.h:300-306; the TAG of -M DTM, Receiver.cpp:26-66).  version, status,
- * rxtime_us, toa_us, include_ssl, uuid and suffix stay the output's, and so do the COMMUNITY_HUB and NMEA_TAG counters (per engine).
+ * rxtime_us (each frame's stamp on an engine with a clock), toa_us, include_ssl, uuid and suffix stay the output's, and so do the
+ * COMMUNITY_HUB and NMEA_TAG counters (per engine).
  * counters[5] / [6] keep counting each stream's first and second channel, whatever its letters.  So the records expected for stream s
  * are exactly aisgpu_msg_format(frame, tag of s, ...).
  *
@@ -465,6 +466,44 @@ int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int 
  * every product and sum rounded to float.  f = 0: out = v.  The engine computes the same bits on the GPU.  0, or AISGPU_EINVAL for an
  * unknown format, sample_rate < 1, first_sample < 0, n < 0, null buffers, or an offset outside (-fs/2, fs/2). */
 int aisgpu_tune_restate(int format, int sample_rate, int32_t offset_hz, int64_t first_sample, const void *in, int64_t n, void *out_cf32);
+
+/* ---- Receive time: a clock per stream (DESIGN.md 7e) ----
+ *
+ * Without a clock every record the engine formats prints the output's aisgpu_tag.rxtime_us.  aisgpu_set_clock stamps every frame
+ * with its own receive time instead, at the reference's granularity: its decoder thread stamps a message (Message::Stamp,
+ * AIS.cpp:76-77) while it processes the block that completes it, so here a frame's stamp is a function of its stream s and of
+ * aisgpu_msg.chunk, the submit c that completed it:
+ *   - recording clock (start_us != NULL; start_us[s] = the time of stream s's first sample, microseconds since the epoch):
+ *     stamp(s, c) = start_us[s] + floor(S_c * 10^6 / fs), computed as q * 10^6 + (r * 10^6) / fs with q = S_c / fs, r = S_c % fs.
+ *     S_c is the number of samples per stream submitted through submit c inclusive (counters[2] right after it) and fs the config's
+ *     sample_rate (F32_FS4: the rate of the real samples; AISGPU_MODEL_DISCRIMINATOR: the audio rate).  Submit lengths may vary;
+ *     the zero-padded tail blocks of aisgpu_feed_files / aisgpu_feed_wav_files are submits and count as signal time;
+ *   - live clock (start_us == NULL): every stream's stamp for submit c is std::chrono::system_clock's time in microseconds since
+ *     the epoch, as Message::Stamp reads it, read once by the aisgpu_submit* call (or feeder block) that made submit c, between
+ *     that call's entry and its return.
+ * The record of every published frame, in every format and on every path (aisgpu_poll_lines, aisgpu_poll_json, the feeders'
+ * polls), is then exactly aisgpu_msg_format(frame, tag', ...), tag' being the record's tag (the output's, or its stream's with a
+ * receiver table) with rxtime_us = the frame's stamp.  Mode bit 1 still decides, per stream, whether the JSON formats and FULL
+ * print the time; NMEA_TAG, BINARY_NMEA and COMMUNITY_HUB print it always.  aisgpu_poll's frames are unchanged (aisgpu_msg has no
+ * time): aisgpu_stamp(h, frame.stream, frame.chunk) gives it.
+ *
+ * Rules (AISGPU_EINVAL with the reason in aisgpu_last_error(h), the handle untouched): n == n_streams, also for start_us == NULL;
+ * before the first submit; at most once; every start_us[s] in [0, 253402300800000000) (before 10000-01-01, so that rxtime stays
+ * YYYYMMDDHHMMSS).  Refused on a group member: the leader's clock stamps the whole group's frames (as the leader's tuning tunes
+ * the rows the group reads), and a member's records and aisgpu_stamp follow the leader's submits.  It may come before or after
+ * aisgpu_lines_enable / aisgpu_json_enable and aisgpu_set_receivers.
+ *
+ * Memory: 8 bytes of host memory per submit for the life of the engine (S_c or the wall time, shared by a group), plus the start
+ * times (8 bytes per stream); with a format enabled, a device buffer of one 8-byte stamp per frame of a 4096-frame batch (32 KB),
+ * uploaded beside the frames.  Without a clock nothing of this is allocated, uploaded or launched.  (The record slots of every
+ * engine hold the longest time members any stamp can print.) */
+int aisgpu_set_clock(aisgpu_handle *h, const int64_t *start_us, int n);
+/* The rules of aisgpu_set_clock that need no device, for an engine created with *cfg: 0, or AISGPU_EINVAL with the reason in
+ * aisgpu_last_error(NULL). */
+int aisgpu_check_clock(const aisgpu_config *cfg, const int64_t *start_us, int n);
+/* *rxtime_us = the stamp of the frames of stream `stream` completed by submit `chunk` (aisgpu_msg.chunk), for any submit made so far
+ * (a member: its leader's submits).  AISGPU_EINVAL without a clock, and for a stream or chunk out of range. */
+int aisgpu_stamp(aisgpu_handle *h, int stream, int64_t chunk, int64_t *rxtime_us);
 
 /* == AIS::Message::getBinaryNMEA(out, tag, crc) (Message.cpp:277-396): 0xAC 0x00 framed, byte-stuffed binary record with an
  * optional CRC-16 (Helper.cpp:42-57).  Returns the bytes written, 0 when the reference would emit nothing. Host-only. */
