@@ -28,7 +28,7 @@ EXPORTS = ["aisgpu_abi_version", "aisgpu_default_config", "aisgpu_create", "aisg
            "aisgpu_msg_json_full", "aisgpu_json_enable", "aisgpu_poll_json", "aisgpu_msg_format", "aisgpu_lines_enable",
            "aisgpu_poll_lines", "aisgpu_set_receivers", "aisgpu_check_receivers",
            "aisgpu_set_tuning", "aisgpu_check_tuning", "aisgpu_tune_restate", "aisgpu_set_clock", "aisgpu_check_clock",
-           "aisgpu_stamp"]
+           "aisgpu_stamp", "aisgpu_set_tunings", "aisgpu_check_tunings"]
 
 OK, EINVAL, ENODEV, ECUDA, ENOMEM, EOVERFLOW, EIO = 0, -1, -2, -3, -4, -5, -6
 # message formats: positions in the reference's enum class MessageFormat (MSGFORMAT of its outputs); include/aisgpu.h describes each record
@@ -97,11 +97,11 @@ def _offsets(offsets):
     return (C.c_int32 * max(len(offsets), 1))(*[int(f) for f in offsets])
 
 
-def check_tuning(offsets, **engine):
-    """aisgpu_check_tuning (no GPU needed): the rules of Engine.set_tuning for an engine of keyword arguments `engine`.
-    Raises with the reason if the offsets (Hz, one per stream) would be refused."""
+def check_tuning(offsets, per_input=1, **engine):
+    """aisgpu_check_tunings (no GPU needed): the rules of Engine.set_tuning for an engine of keyword arguments `engine`.
+    Raises with the reason if the offsets (Hz, one per stream), per_input tunings of each input, would be refused."""
     lib = load()
-    rc = lib.aisgpu_check_tuning(C.byref(make_config(**engine)), _offsets(offsets), len(offsets))
+    rc = lib.aisgpu_check_tunings(C.byref(make_config(**engine)), _offsets(offsets), len(offsets), int(per_input))
     if rc:
         raise AisGpuError("rc=%d: %s" % (rc, lib.aisgpu_last_error(None).decode("latin-1")))
 
@@ -128,8 +128,7 @@ def tune_restate(fmt, sample_rate, offset_hz, first_sample, samples):
     offset_hz -> complex64 array: what a tuned engine's rows after the tune hold."""
     lib = load()
     a = np.ascontiguousarray(samples)
-    bps = {FMT_CF32: 8, FMT_CU8: 2, FMT_CS8: 2, FMT_CS16: 4, FMT_F32_FS4: 4, FMT_DC16H: 12}[fmt]
-    n = a.nbytes // bps
+    n = a.nbytes // BPS[fmt]
     out = np.empty(n, np.complex64)
     rc = lib.aisgpu_tune_restate(int(fmt), int(sample_rate), int(offset_hz), int(first_sample), a.ctypes.data_as(C.c_void_p), n,
                                  out.ctypes.data_as(C.c_void_p))
@@ -137,6 +136,8 @@ def tune_restate(fmt, sample_rate, offset_hz, first_sample, samples):
         raise AisGpuError("aisgpu_tune_restate rc=%d" % rc)
     return out
 
+
+BPS = {FMT_CF32: 8, FMT_CU8: 2, FMT_CS8: 2, FMT_CS16: 4, FMT_F32_FS4: 4, FMT_DC16H: 12}  # bytes per sample of each input format
 
 MSG_FN = C.CFUNCTYPE(None, C.POINTER(MsgStruct), C.c_int, C.c_void_p)
 
@@ -228,6 +229,9 @@ def load():
         lib.aisgpu_set_tuning.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int]
         lib.aisgpu_check_tuning.argtypes = [C.POINTER(Config), C.POINTER(C.c_int32), C.c_int]
         lib.aisgpu_tune_restate.argtypes = [C.c_int, C.c_int, C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
+    if hasattr(lib, "aisgpu_set_tunings"):  # absent from libraries built before several tunings of one input (AISGPU_LIB)
+        lib.aisgpu_set_tunings.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.c_int, C.c_int]
+        lib.aisgpu_check_tunings.argtypes = [C.POINTER(Config), C.POINTER(C.c_int32), C.c_int, C.c_int]
     if hasattr(lib, "aisgpu_set_clock"):  # absent from libraries built before the clocks (AISGPU_LIB)
         lib.aisgpu_set_clock.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.c_int]
         lib.aisgpu_check_clock.argtypes = [C.POINTER(Config), C.POINTER(C.c_int64), C.c_int]
@@ -430,6 +434,7 @@ class Engine:
         if rc:
             raise AisGpuError("aisgpu_create rc=%d: %s" % (rc, self.lib.aisgpu_last_error(None).decode()))
         self.n_streams = n_streams
+        self.inputs = n_streams  # the rows every submit holds: n_streams / per_input after set_tuning
         self.fmt = fmt
         self.overflows = 0  # polls that reported AISGPU_EOVERFLOW (frames were dropped; the survivors were delivered)
 
@@ -451,7 +456,7 @@ class Engine:
         m = Engine.__new__(Engine)
         m.lib, m.kwargs, m.cfg, m.h = self.lib, kw, cfg, h
         m.leader = self  # keeps the leader alive while the member exists
-        m.n_streams, m.fmt, m.overflows = self.n_streams, self.fmt, 0
+        m.n_streams, m.inputs, m.fmt, m.overflows = self.n_streams, self.inputs, self.fmt, 0
         return m
 
     def _chk(self, rc):
@@ -461,17 +466,27 @@ class Engine:
         if rc:
             raise AisGpuError("rc=%d: %s" % (rc, self.lib.aisgpu_last_error(self.h).decode()))
 
+    def _check_rows(self, what, rows):
+        if rows != self.inputs:
+            raise ValueError("%s: %d rows for an engine of %d inputs (n_streams %d)" % (what, rows, self.inputs, self.n_streams))
+
     def submit(self, host_array, n_samples):
-        """host_array: contiguous numpy array holding n_streams x n_samples samples (stream-major)."""
+        """host_array: contiguous numpy array holding inputs x n_samples samples (input-major; inputs is n_streams unless
+        set_tuning gave each input several tunings)."""
         a = np.ascontiguousarray(host_array)
+        if a.ndim >= 2:
+            self._check_rows("submit", a.shape[0])
+        if a.nbytes < self.inputs * n_samples * BPS[self.fmt]:
+            raise ValueError("submit: %d bytes for %d inputs x %d samples" % (a.nbytes, self.inputs, n_samples))
         self._chk(self.lib.aisgpu_submit(self.h, a.ctypes.data_as(C.c_void_p), n_samples))
 
     def submit_ptr(self, host_ptr, n_samples):
         self._chk(self.lib.aisgpu_submit(self.h, C.c_void_p(host_ptr), n_samples))
 
     def submit_v(self, host_arrays, n_samples):
-        """One host array per stream (the shape n_streams independent receivers deliver)."""
+        """One host array per input (the shape independent receivers deliver)."""
         arrs = [np.ascontiguousarray(a) for a in host_arrays]
+        self._check_rows("submit_v", len(arrs))
         ptrs = (C.c_void_p * len(arrs))(*[a.ctypes.data for a in arrs])
         self._chk(self.lib.aisgpu_submit_v(self.h, ptrs, n_samples))
 
@@ -482,16 +497,16 @@ class Engine:
         return t.value
 
     def feed_files(self, paths, n):
-        """aisgpu_feed_files: one recording per stream, blocks of n samples; returns (messages, blocks submitted)."""
+        """aisgpu_feed_files: one recording per input, blocks of n samples; returns (messages, blocks submitted)."""
         return self._feed(self.lib.aisgpu_feed_files, paths, n)
 
     def feed_wav_files(self, paths, n):
-        """aisgpu_feed_wav_files: one WAV recording per stream, in the engine's format and at its rate, read from its data chunk
+        """aisgpu_feed_wav_files: one WAV recording per input, in the engine's format and at its rate, read from its data chunk
         to its end in blocks of n samples; returns (messages, blocks submitted)."""
         return self._feed(self.lib.aisgpu_feed_wav_files, paths, n)
 
     def _feed(self, f, paths, n):
-        assert len(paths) == self.n_streams
+        self._check_rows(f.__name__, len(paths))
         arr = (C.c_char_p * len(paths))(*[os.fsencode(p) for p in paths])
         out = []
         cb = MSG_FN(lambda msgs, k, user: out.extend(Msg(msgs[i]) for i in range(k)))
@@ -538,7 +553,11 @@ class Engine:
         self._chk(self.lib.aisgpu_allreduce_counts(self.h, c))
         return list(c)
 
-    def submit_device(self, dev_ptr, stride_samples, n_samples):
+    def submit_device(self, dev_ptr, stride_samples, n_samples, rows=None):
+        """aisgpu_submit_device: `inputs` rows of the engine's format, stride_samples apart, from dev_ptr.  rows: how many rows the
+        caller's batch holds, checked against inputs when given."""
+        if rows is not None:
+            self._check_rows("submit_device", rows)
         self._chk(self.lib.aisgpu_submit_device(self.h, C.c_void_p(dev_ptr), stride_samples, n_samples))
 
     def sync(self):
@@ -577,10 +596,12 @@ class Engine:
         self._receivers = receiver_table(receivers)  # copied by the library; kept anyway
         self._chk(self.lib.aisgpu_set_receivers(self.h, self._receivers, len(receivers)))
 
-    def set_tuning(self, offsets):
-        """aisgpu_set_tuning: one offset in Hz per stream (the channel pair's centre, or in X mode the channel, relative to the
-        capture's centre), before the first submit and at most once.  Each submit is then mixed on the GPU so that it lands at 0 Hz."""
-        self._chk(self.lib.aisgpu_set_tuning(self.h, _offsets(offsets), len(offsets)))
+    def set_tuning(self, offsets, per_input=1):
+        """aisgpu_set_tunings: one offset in Hz per stream (the channel pair's centre, or in X mode the channel, relative to the
+        capture's centre), before the first submit and at most once.  Each submit is then mixed on the GPU so that it lands at 0 Hz.
+        per_input > 1: each input row feeds per_input adjacent streams, and every submit and feed takes n_streams / per_input rows."""
+        self._chk(self.lib.aisgpu_set_tunings(self.h, _offsets(offsets), len(offsets), int(per_input)))
+        self.inputs = self.n_streams // int(per_input)
 
     def set_clock(self, start_us=None):
         """aisgpu_set_clock: start_us, one start time per stream in microseconds since the epoch (a recording clock), or None (the

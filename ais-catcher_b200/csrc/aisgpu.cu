@@ -281,11 +281,13 @@ struct aisgpu_handle {
 	std::vector<int> seq; // per-stream multi-sentence sequence id (Message.cpp:28-39 is process-global in the reference)
 	std::vector<Receiver> rx; // per stream: the config's fields, or the receiver aisgpu_set_receivers installed
 	bool rx_table = false;    // aisgpu_set_receivers has been called: the records take the receivers' TAG fields
-	// The per-stream digital tune (aisgpu_set_tuning, tune.cu).  With a table every submit first runs k_tune on fe_stream: the
-	// caller's samples, converted and mixed by each stream's offset, into d_tune [n_streams][tune_stride] as CF32, which everything
-	// behind it then reads as a CF32 input (src_fmt); behind a resampler with no CIC stage (kA = 0) k_tune writes D0 directly and is
-	// the pre-stage's conversion.  Without a table nothing of this is allocated or launched.
+	// The per-stream digital tune (aisgpu_set_tunings, tune.cu).  With a table every submit first runs k_tune on fe_stream: the
+	// caller's n_streams / per_input input rows, converted and mixed by each stream's offset (input row r feeds streams
+	// r * per_input .. r * per_input + per_input - 1), into d_tune [n_streams][tune_stride] as CF32, which everything behind it then
+	// reads as a CF32 input (src_fmt); behind a resampler with no CIC stage (kA = 0) k_tune writes D0 directly and is the pre-stage's
+	// conversion.  Without a table nothing of this is allocated or launched, and per_input is 1.
 	bool tuned = false;
+	int per_input = 1;
 	float2 *d_tune = nullptr, *d_tune_tab = nullptr;
 	long long tune_stride = 0;
 	int *d_tune_fk = nullptr;
@@ -472,6 +474,9 @@ bool has_cic(const aisgpu_handle *h) { return h->pre_us || h->kA > 0; }
 
 // The format the first stage reads: the caller's, or the CF32 rows of the tune (aisgpu_set_tuning)
 int src_fmt(const aisgpu_handle *h) { return h->tuned ? AISGPU_FMT_CF32 : h->cfg.format; }
+
+// The rows the caller's submits hold: one per stream, or one per per_input streams behind a fan of tunings (aisgpu_set_tunings)
+int inputs(const aisgpu_handle *h) { return h->cfg.n_streams / h->per_input; }
 
 // A tuned engine whose CIC stage would only convert (a resampler behind no CIC stage): the tune writes D0 in its place
 bool tune_into_d0(const aisgpu_handle *h) { return h->tuned && h->pre_us && h->kA == 0; }
@@ -1477,8 +1482,9 @@ int check_placement(aisgpu_handle *h, const void *dev, int64_t stride) {
 
 int mark_ticket(aisgpu_handle *h, long long t);
 
-// The tune stage (aisgpu_set_tuning): the caller's N samples per stream, sample 0 being sample counters[2] of every stream, converted
-// and mixed into d_tune (or into D0, tune_into_d0); what follows reads d_tune in place of the caller's rows.
+// The tune stage (aisgpu_set_tunings): the caller's N samples per input row, sample 0 being sample counters[2] of every stream,
+// converted and mixed into the rows of the row's streams in d_tune (or in D0, tune_into_d0); what follows reads d_tune in place of the
+// caller's rows.
 int tune_input(aisgpu_handle *h, const void *&dev_in, long long &stride, int N) {
 	TuneParams p;
 	p.in = dev_in;
@@ -1487,7 +1493,8 @@ int tune_input(aisgpu_handle *h, const void *&dev_in, long long &stride, int N) 
 	p.out_stride = h->d_tune ? h->tune_stride : h->d0_stride;
 	p.out_off = h->d_tune ? 0 : 2;
 	p.N = N;
-	p.B = h->cfg.n_streams;
+	p.R = inputs(h);
+	p.T = h->per_input;
 	p.fs = h->cfg.sample_rate;
 	p.tab_len = tune_table_len(p.fs);
 	p.first = (long long)h->counters[2];
@@ -1833,6 +1840,7 @@ const char *aisgpu_last_error(aisgpu_handle *h) { return h ? h->err.c_str() : g_
 
 // hooks for the host-only units of the library (host_internal.h)
 const aisgpu_config *aisgpu_internal_config(aisgpu_handle *h) { return &h->cfg; }
+int aisgpu_internal_inputs(aisgpu_handle *h) { return inputs(h); }
 void aisgpu_internal_set_error(aisgpu_handle *h, const char *msg) { (h ? h->err : g_create_error) = msg; }
 int aisgpu_internal_grouped(aisgpu_handle *h) { return h->member || !h->members.empty(); }
 
@@ -2112,28 +2120,28 @@ int aisgpu_submit_device(aisgpu_handle *h, const void *dev_samples, int64_t stri
 	return poison(h, submit_outer(h, dev_samples, stride_samples, n_samples));
 }
 
-// Host submits: the batch goes through one of two device staging buffers (copy stream), the front end of the submit
-// before last being the previous reader of that buffer.  `ptrs` != nullptr: one host pointer per stream.
+// Host submits: the batch (one row per input, inputs(h)) goes through one of two device staging buffers (copy stream), the front end
+// of the submit before last being the previous reader of that buffer.  `ptrs` != nullptr: one host pointer per input row.
 static int submit_host(aisgpu_handle *h, const void *host_samples, const void *const *ptrs, int n_samples, bool wait_copy, int64_t *ticket) {
 	if (int rc = check_outer(h, n_samples)) return rc;
 	const size_t row_bytes = (size_t)n_samples * h->obps;
-	const int cur = h->in_cur;
+	const int cur = h->in_cur, R = inputs(h);
 	if (!h->d_in[cur]) {
-		if (int rc = dalloc(h, &h->d_in[cur], (size_t)h->cfg.n_streams * h->cfg.max_chunk_samples * h->obps)) return rc;
+		if (int rc = dalloc(h, &h->d_in[cur], (size_t)R * h->cfg.max_chunk_samples * h->obps)) return rc;
 		CU(cudaStreamSynchronize(h->stream)); // dalloc clears on h->stream
 	}
 	if (h->in_used[cur]) CU(cudaStreamWaitEvent(h->copy_stream, h->ev_done[cur], 0));
 	if (ptrs) {
-		for (int s = 0; s < h->cfg.n_streams; s++) {
+		for (int s = 0; s < R; s++) {
 			if (!ptrs[s]) {
 				h->err = "null stream pointer";
 				return AISGPU_EINVAL;
 			}
 		}
-		for (int s = 0; s < h->cfg.n_streams; s++)
+		for (int s = 0; s < R; s++)
 			CU(cudaMemcpyAsync(h->d_in[cur] + (size_t)s * row_bytes, ptrs[s], row_bytes, cudaMemcpyHostToDevice, h->copy_stream));
 	}
-	else CU(cudaMemcpyAsync(h->d_in[cur], host_samples, row_bytes * h->cfg.n_streams, cudaMemcpyHostToDevice, h->copy_stream));
+	else CU(cudaMemcpyAsync(h->d_in[cur], host_samples, row_bytes * R, cudaMemcpyHostToDevice, h->copy_stream));
 	CU(cudaEventRecord(h->ev_copy[cur], h->copy_stream));
 	CU(cudaStreamWaitEvent(h->fe_stream, h->ev_copy[cur], 0));
 	if (ticket) *ticket = (int64_t)h->counters[3];
@@ -2450,10 +2458,13 @@ int aisgpu_set_receivers(aisgpu_handle *h, const aisgpu_receiver *r, int n) {
 
 namespace {
 
-// The rules of aisgpu_set_tuning that need no device: "" or the reason.  fp_ds: the engine runs the integer CIC front end.
-std::string tuning_refusal(const aisgpu_config &c, bool fp_ds, const int32_t *f, int n) {
+// The rules of aisgpu_set_tunings that need no device: "" or the reason.  fp_ds: the engine runs the integer CIC front end.
+std::string tuning_refusal(const aisgpu_config &c, bool fp_ds, const int32_t *f, int n, int per_input) {
 	if (!f) return "aisgpu_set_tuning: null offset table";
 	if (n != c.n_streams) return "aisgpu_set_tuning: " + std::to_string(n) + " offsets for " + std::to_string(c.n_streams) + " streams";
+	if (per_input < 1 || c.n_streams % per_input)
+		return "aisgpu_set_tunings: per_input " + std::to_string(per_input) + " must be at least 1 and divide n_streams " +
+			   std::to_string(c.n_streams);
 	if (c.model == AISGPU_MODEL_DISCRIMINATOR)
 		return "aisgpu_set_tuning: the FM-discriminator input model reads I and Q as two real audio channels: there is nothing to tune";
 	if (fp_ds) return "aisgpu_set_tuning: FP_DS on: the integer front end reads the caller's CU8 samples directly and cannot take tuned ones";
@@ -2467,7 +2478,7 @@ std::string tuning_refusal(const aisgpu_config &c, bool fp_ds, const int32_t *f,
 
 } // namespace
 
-int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int n) {
+int aisgpu_check_tunings(const aisgpu_config *cfg, const int32_t *offset_hz, int n, int per_input) {
 	aisgpu_config c;
 	if (!copy_config(cfg, &c)) {
 		g_create_error = "aisgpu_check_tuning: null config or struct_size mismatch";
@@ -2476,7 +2487,7 @@ int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int 
 	// plan_frontend's FP_DS condition: the exact 1536K bucket of AB mode fed CU8
 	const bool fp_ds = c.fp_ds && c.channel_mode == AISGPU_MODE_AB && c.model != AISGPU_MODEL_DISCRIMINATOR && c.sample_rate == 1536000 &&
 					   c.format == AISGPU_FMT_CU8;
-	const std::string why = tuning_refusal(c, fp_ds, offset_hz, n);
+	const std::string why = tuning_refusal(c, fp_ds, offset_hz, n, per_input);
 	if (!why.empty()) {
 		g_create_error = why;
 		return AISGPU_EINVAL;
@@ -2484,9 +2495,11 @@ int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int 
 	return 0;
 }
 
-int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) {
+int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int n) { return aisgpu_check_tunings(cfg, offset_hz, n, 1); }
+
+int aisgpu_set_tunings(aisgpu_handle *h, const int32_t *offset_hz, int n, int per_input) {
 	ENTER(h);
-	std::string why = tuning_refusal(h->given, h->fp_ds != 0, offset_hz, n);
+	std::string why = tuning_refusal(h->given, h->fp_ds != 0, offset_hz, n, per_input);
 	if (why.empty() && h->member)
 		why = "aisgpu_set_tuning: this engine is a member of a group and reads its leader's front end: install the table on the leader";
 	if (why.empty() && h->tuned) why = "aisgpu_set_tuning: a tuning table is already installed";
@@ -2499,6 +2512,7 @@ int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) {
 	// plan only differs in the format it reads and the warm-up history that follows from it), and give the warm-up histories CF32 size.
 	const int B = h->cfg.n_streams, fs = h->cfg.sample_rate;
 	h->tuned = true;
+	h->per_input = per_input;
 	if (int rc = plan_frontend(h)) return poison(h, rc == AISGPU_EINVAL ? AISGPU_ECUDA : rc);
 	h->bps = bytes_per_sample(h->in_fmt);
 	h->pbps = bytes_per_sample(AISGPU_FMT_CF32);
@@ -2509,6 +2523,11 @@ int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) {
 		if (h->d_raw_tail[i]) {
 			dfree(h, h->d_raw_tail[i]);
 			if (int rc = dalloc(h, &h->d_raw_tail[i], (size_t)B * raw_tail_len(h) * h->pbps)) return poison(h, rc);
+		}
+		// host staging allocated at creation holds one row per stream; no submit has used it yet: one row per input from now on
+		if (h->d_in[i] && per_input > 1) {
+			dfree(h, h->d_in[i]);
+			if (int rc = dalloc(h, &h->d_in[i], (size_t)inputs(h) * h->cfg.max_chunk_samples * h->obps)) return poison(h, rc);
 		}
 	}
 	if (!tune_into_d0(h)) {
@@ -2530,6 +2549,8 @@ int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) {
 	h->tune_ctas = 4 * sms;
 	return 0;
 }
+
+int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n) { return aisgpu_set_tunings(h, offset_hz, n, 1); }
 
 namespace {
 

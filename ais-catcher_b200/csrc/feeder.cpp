@@ -1,4 +1,5 @@
-// Ingest (SURVEY.md 8f rank 4): n_streams recorded IQ files feeding one engine -- the batch form of the reference's
+// Ingest (SURVEY.md 8f rank 4): one recorded IQ file per input row feeding one engine (n_streams of them, or n_streams / per_input
+// behind a fan of tunings, aisgpu_set_tunings) -- the batch form of the reference's
 // Device::RAWFile (Source/Device/FileRAW.cpp:36-165): each file is read in fixed blocks, the last block of a file is
 // zero-padded (FileRAW.cpp:91-94), and the stream of blocks ends when the longest file has been consumed (shorter files
 // keep delivering zeros, which is what a silent receiver looks like to the models).  WAV recordings are read the same way
@@ -29,7 +30,7 @@ struct Source {
 	bool eof = false;
 };
 
-// reads one block of every stream in [s0, s1) into dst (stream-major); returns through `live` whether any file still had data
+// reads one block of every input in [s0, s1) into dst (input-major); returns through `live` whether any file still had data
 void read_block(std::vector<Source> &src, int s0, int s1, unsigned char *dst, size_t block_bytes, std::atomic<int> &live) {
 	for (int s = s0; s < s1; s++) {
 		unsigned char *p = dst + (size_t)s * block_bytes;
@@ -56,12 +57,12 @@ int check_args(aisgpu_handle *h, const char *who, const char *const *paths, int 
 	return 0;
 }
 
-// The blocks of every stream, stream s read from byte offsets[s] of paths[s] (offsets == NULL: from the start) to its end.
+// The blocks of every input row, row s read from byte offsets[s] of paths[s] (offsets == NULL: from the start) to its end.
 int feed(aisgpu_handle *h, const char *who, const char *const *paths, const int64_t *offsets, int n_samples, aisgpu_msg_fn fn, void *user,
 		 uint64_t *n_blocks) {
 	if (int rc = check_args(h, who, paths, n_samples)) return rc;
 	const aisgpu_config *cfg = aisgpu_internal_config(h);
-	const int B = cfg->n_streams;
+	const int B = aisgpu_internal_inputs(h);
 	const size_t bps = cfg->format == AISGPU_FMT_CF32 ? 8 : (cfg->format == AISGPU_FMT_DC16H ? 12 : ((cfg->format == AISGPU_FMT_CS16 || cfg->format == AISGPU_FMT_F32_FS4) ? 4 : 2));
 	const size_t block_bytes = (size_t)n_samples * bps;
 	std::vector<Source> src((size_t)B);
@@ -91,7 +92,7 @@ int feed(aisgpu_handle *h, const char *who, const char *const *paths, const int6
 			return AISGPU_ENOMEM;
 		}
 	const int T = (int)std::max(1u, std::min(std::min(std::thread::hardware_concurrency(), 16u), (unsigned)B));
-	auto fill = [&](unsigned char *dst) { // one block of every stream, files shared out over T threads; false once all files are drained
+	auto fill = [&](unsigned char *dst) { // one block of every input, files shared out over T threads; false once all files are drained
 		std::atomic<int> live(0);
 		std::vector<std::thread> th;
 		for (int t = 1; t < T; t++) th.emplace_back(read_block, std::ref(src), (int)((long long)B * t / T), (int)((long long)B * (t + 1) / T), dst, block_bytes, std::ref(live));
@@ -230,8 +231,9 @@ extern "C" int aisgpu_feed_wav_files(aisgpu_handle *h, const char *const *paths,
 	const char *who = "aisgpu_feed_wav_files";
 	if (int rc = check_args(h, who, paths, n_samples)) return rc;
 	const aisgpu_config *cfg = aisgpu_internal_config(h);
-	std::vector<int64_t> offsets((size_t)cfg->n_streams);
-	for (int s = 0; s < cfg->n_streams; s++) {
+	const int B = aisgpu_internal_inputs(h);
+	std::vector<int64_t> offsets((size_t)B);
+	for (int s = 0; s < B; s++) {
 		const std::string name = std::string(who) + ": \"" + (paths[s] ? paths[s] : "(null)") + "\": ";
 		int32_t fmt = 0;
 		uint32_t rate = 0;

@@ -211,16 +211,17 @@ cudaError_t set_taps_bh28_3(const float *taps26);
 constexpr int GROUP_MAX = 8; // engines in one group, the leader included
 cudaError_t launch_c_fanout(const float2 *src, long long src_stride, int src_off, float2 *const *dst, int nd, long long dst_stride, int dst_off, int n,
 							int rows, cudaStream_t s);
-// tune.cu: the per-stream digital tune (aisgpu_set_tuning).  Rows of N samples in format fmt (in_stride samples apart) -> CF32 rows of
-// out (out_stride apart, from element out_off); sample i of the submit is sample first + i of its stream; fk[s]: stream s's offset
-// modulo fs in [0, fs) (0: converted only); tab: tune_tables(fs), tab_len = tune_table_len(fs) entries.  At most `ctas` CTAs.
+// tune.cu: the per-stream digital tune (aisgpu_set_tunings).  R input rows of N samples in format fmt (in_stride samples apart) -> R * T
+// CF32 rows of out (out_stride apart, from element out_off), input row r feeding streams rT .. rT + T - 1; sample i of the submit is
+// sample first + i of its stream; fk[s]: stream s's offset modulo fs in [0, fs) (0: converted only); tab: tune_tables(fs), tab_len =
+// tune_table_len(fs) entries.  At most `ctas` CTAs.
 struct TuneParams {
 	const void *in;
 	long long in_stride;
 	float2 *out;
 	long long out_stride;
 	int out_off;
-	int N, B, fs, tab_len;
+	int N, R, T, fs, tab_len;
 	long long first;
 	const int *fk;
 	const float2 *tab;

@@ -1,5 +1,6 @@
-// tune.cu -- the per-stream digital tune (aisgpu_set_tuning): ConvertRAW of the caller's samples, multiplied by the conjugate of a
-// phasor at the stream's offset, into CF32 rows that the rest of the engine reads as a CF32 input.
+// tune.cu -- the per-stream digital tune (aisgpu_set_tunings): ConvertRAW of the caller's samples, multiplied by the conjugate of a
+// phasor at the stream's offset, into CF32 rows that the rest of the engine reads as a CF32 input.  Each input row feeds T adjacent
+// streams, each with its own offset.
 //
 // The definition (include/aisgpu.h, aisgpu_tune_restate): sample n of a stream (counted from its first sample, across submits) with
 // offset f and sample rate fs has the phase index k = ((n mod fs) * f) mod fs in [0, fs); k = a * 4096 + b; p = T_hi[a] * T_lo[b] with
@@ -88,9 +89,10 @@ constexpr int TUNE_LO = 4096;
 
 constexpr int TUNE_THREADS = 256, TUNE_RUN = 8; // a CTA visits TUNE_THREADS * TUNE_RUN samples of one row at a time
 
-// One read of the input and one 8-byte write per sample.  Each CTA copies the tables into shared memory once and then walks work
-// items (row, segment of TUNE_THREADS * TUNE_RUN samples); thread t takes samples t, t + 256, ... of the segment, so every load and
-// store is coalesced, and steps k by 256 * f mod fs from one to the next.
+// One read of the input and one 8-byte write per sample and tuning.  Each CTA copies the tables into shared memory once and then walks
+// work items (input row r, segment of TUNE_THREADS * TUNE_RUN samples); thread t converts samples t, t + 256, ... of the segment once,
+// then mixes them by each of the row's T streams rT .. rT + T - 1 in turn and stores them to that stream's row, so every load and store
+// is coalesced.  Within a stream k steps by 256 * f mod fs from one sample to the next.
 template <int FMT>
 __global__ void __launch_bounds__(TUNE_THREADS) k_tune(TuneParams p) {
 	extern __shared__ float2 tune_tab[];
@@ -98,31 +100,37 @@ __global__ void __launch_bounds__(TUNE_THREADS) k_tune(TuneParams p) {
 	__syncthreads();
 	constexpr int SEG = TUNE_THREADS * TUNE_RUN;
 	const int segs = (p.N + SEG - 1) / SEG;
-	for (long long w = blockIdx.x; w < (long long)segs * p.B; w += gridDim.x) {
-		const int s = (int)(w / segs), i0 = (int)(w % segs) * SEG + threadIdx.x;
-		const int fk = p.fk[s];
-		const void *row = reinterpret_cast<const unsigned char *>(p.in) + (long long)s * p.in_stride * fe_fmt_bps(FMT);
-		float2 *out = p.out + (long long)s * p.out_stride + p.out_off;
+	for (long long w = blockIdx.x; w < (long long)segs * p.R; w += gridDim.x) {
+		const int r = (int)(w / segs), i0 = (int)(w % segs) * SEG + threadIdx.x;
+		const void *row = reinterpret_cast<const unsigned char *>(p.in) + (long long)r * p.in_stride * fe_fmt_bps(FMT);
 		float2 v[TUNE_RUN] = {};
 #pragma unroll
 		for (int j = 0; j < TUNE_RUN; j++) {
 			const int i = i0 + j * TUNE_THREADS;
 			if (i < p.N) v[j] = tune_convert(FMT, row, i, p.first + i);
 		}
-		if (fk) {
-			unsigned k = tune_k(p.first + i0, fk, p.fs);
-			const unsigned dk = (unsigned)((long long)TUNE_THREADS * fk % p.fs);
+#pragma unroll 1
+		for (int s = r * p.T; s < (r + 1) * p.T; s++) {
+			const int fk = p.fk[s];
+			float2 *out = p.out + (long long)s * p.out_stride + p.out_off;
+			if (fk) {
+				unsigned k = tune_k(p.first + i0, fk, p.fs);
+				const unsigned dk = (unsigned)((long long)TUNE_THREADS * fk % p.fs);
 #pragma unroll
-			for (int j = 0; j < TUNE_RUN; j++) {
-				v[j] = tune_mix(v[j], tune_tab[TUNE_LO + (k >> 12)], tune_tab[k & (TUNE_LO - 1)]);
-				k += dk;
-				if (k >= (unsigned)p.fs) k -= p.fs;
+				for (int j = 0; j < TUNE_RUN; j++) {
+					const int i = i0 + j * TUNE_THREADS;
+					if (i < p.N) out[i] = tune_mix(v[j], tune_tab[TUNE_LO + (k >> 12)], tune_tab[k & (TUNE_LO - 1)]);
+					k += dk;
+					if (k >= (unsigned)p.fs) k -= p.fs;
+				}
 			}
-		}
+			else {
 #pragma unroll
-		for (int j = 0; j < TUNE_RUN; j++) {
-			const int i = i0 + j * TUNE_THREADS;
-			if (i < p.N) out[i] = v[j];
+				for (int j = 0; j < TUNE_RUN; j++) {
+					const int i = i0 + j * TUNE_THREADS;
+					if (i < p.N) out[i] = v[j];
+				}
+			}
 		}
 	}
 }
@@ -153,7 +161,7 @@ void tune_tables(int fs, float2 *tab) {
 
 cudaError_t launch_tune(const TuneParams &p, int fmt, int ctas, cudaStream_t s) {
 	const int segs = (p.N + TUNE_THREADS * TUNE_RUN - 1) / (TUNE_THREADS * TUNE_RUN);
-	ctas = (int)std::min<long long>((long long)segs * p.B, ctas);
+	ctas = (int)std::min<long long>((long long)segs * p.R, ctas);
 	if (ctas < 1) return cudaSuccess;
 	switch (fmt) {
 	case 0: return launch_tune_f<0>(p, ctas, s);

@@ -35,7 +35,7 @@ extern "C" {
 /* 3 since the engine groups; later additions are new entry points only (the full AIS JSON: aisgpu_msg_json_full, aisgpu_json_enable,
  * aisgpu_poll_json; the output records: aisgpu_msg_format, aisgpu_lines_enable, aisgpu_poll_lines; the receivers:
  * aisgpu_set_receivers, aisgpu_check_receivers; the tuning: aisgpu_set_tuning, aisgpu_check_tuning, aisgpu_tune_restate; the
- * receive time: aisgpu_set_clock, aisgpu_check_clock, aisgpu_stamp), so the number callers check against stays 3.  A caller that
+ * tunings of one input: aisgpu_set_tunings, aisgpu_check_tunings; the receive time: aisgpu_set_clock, aisgpu_check_clock, aisgpu_stamp), so the number callers check against stays 3.  A caller that
  * needs those entry points looks them up (dlsym) instead of relying on the number. */
 #define AISGPU_ABI_VERSION 3
 
@@ -447,16 +447,30 @@ int aisgpu_check_receivers(const aisgpu_config *cfg, const aisgpu_receiver *r, i
  * batches (any stride and base aisgpu_submit_device takes), aisgpu_feed_files and aisgpu_feed_wav_files all go through the tune.
  * A group leader's table tunes the rows its whole group reads.
  *
- * Rules (AISGPU_EINVAL with the reason in aisgpu_last_error(h), the handle untouched): n == n_streams; before the first submit; at most
- * once; -sample_rate/2 < offset_hz[s] < sample_rate/2.  Refused outright: AISGPU_MODEL_DISCRIMINATOR (its I and Q are two real audio
- * channels: nothing to tune), an engine that runs the FP_DS integer front end (it reads CU8 directly), and a group member (its front
- * end is the leader's).
+ * Several tunings of one input (aisgpu_set_tunings, per_input = T > 1): the engine still decodes n_streams streams, but the caller
+ * supplies R = n_streams / T input rows, and stream s reads input row s / T with its own offset offset_hz[s] -- the T tunings of one
+ * input are adjacent streams.  A wideband marine-band capture with T = 2 and offsets +2.6 MHz / -2.6 MHz gives the A/B pair on the even
+ * streams and the C/D pair on the odd ones (their letters come from aisgpu_set_receivers).  Stream s yields exactly what an untuned CF32
+ * engine yields on aisgpu_tune_restate(format, sample_rate, offset_hz[s], 0, input row s / T).  Every entry point that takes the
+ * caller's samples takes R rows: aisgpu_submit / _async (R x n_samples contiguous), aisgpu_submit_v (R pointers),
+ * aisgpu_submit_device (R rows, stride_samples apart, under the same placement rules), aisgpu_feed_files and aisgpu_feed_wav_files (R
+ * paths, file r feeding streams rT .. rT + T - 1).  Everything indexed by stream stays n_streams: receivers, clock starts, dump
+ * prefixes, aisgpu_msg.stream, counters, taps, aisgpu_stamp.  The tune reads each input sample once and writes T CF32 samples.
+ * aisgpu_set_tuning(h, f, n) is aisgpu_set_tunings(h, f, n, 1).
+ *
+ * Rules (AISGPU_EINVAL with the reason in aisgpu_last_error(h), the handle untouched): n == n_streams; per_input >= 1 and divides
+ * n_streams; before the first submit; at most once; -sample_rate/2 < offset_hz[s] < sample_rate/2.  Refused outright:
+ * AISGPU_MODEL_DISCRIMINATOR (its I and Q are two real audio channels: nothing to tune), an engine that runs the FP_DS integer front end
+ * (it reads CU8 directly), and a group member (its front end is the leader's).
  *
  * Memory: the tables (about 36 KB at 1536 kS/s, 56 KB at 12.288 MS/s), and n_streams x max_chunk_samples CF32 samples of scratch,
- * except behind a resampler with no CIC stage in front of it, where the tune writes the resampler's input directly. */
+ * except behind a resampler with no CIC stage in front of it, where the tune writes the resampler's input directly.  The host staging
+ * of aisgpu_submit / _v / _async and the feeders' pinned buffers hold R rows. */
+int aisgpu_set_tunings(aisgpu_handle *h, const int32_t *offset_hz, int n, int per_input);
 int aisgpu_set_tuning(aisgpu_handle *h, const int32_t *offset_hz, int n);
-/* The rules of aisgpu_set_tuning that need no device, for an engine created with *cfg: 0, or AISGPU_EINVAL with the reason in
- * aisgpu_last_error(NULL). */
+/* The rules of aisgpu_set_tunings that need no device, for an engine created with *cfg: 0, or AISGPU_EINVAL with the reason in
+ * aisgpu_last_error(NULL).  aisgpu_check_tuning(cfg, f, n) is aisgpu_check_tunings(cfg, f, n, 1). */
+int aisgpu_check_tunings(const aisgpu_config *cfg, const int32_t *offset_hz, int n, int per_input);
 int aisgpu_check_tuning(const aisgpu_config *cfg, const int32_t *offset_hz, int n);
 /* The definition of the tune, on the host: n samples of one stream in `format` (samples first_sample .. first_sample + n - 1 of it)
  * -> n CF32 samples.  Sample m converts as the reference's ConvertRAW does (F32_FS4's 1, j, -1, -j pattern indexed by m) to v; with

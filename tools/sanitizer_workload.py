@@ -149,4 +149,20 @@ for n in [N, N + 8192, 64 * 5] * (ns // (2 * N + 8192 + 320)):  # locked blocks 
     o += n
 print("slot-locked V2 messages", len(eng.poll()))
 eng.close()
+# two tunings of each input (aisgpu_set_tunings): 3 CU8 inputs feed 6 streams, by host, per-row pointer and device submits
+xf = np.stack([mode_x_util.to_raw(xs[s], aisgpu.FMT_CU8)[0] for s in range(B)])
+eng = aisgpu.Engine(model=aisgpu.MODEL_DEFAULT, sample_rate=fs, fmt=aisgpu.FMT_CU8, n_streams=2 * B, max_chunk=N)
+eng.set_tuning([0, 250000, -300000, 0, 700000, -700000], per_input=2)
+import torch
+xd = torch.from_numpy(np.ascontiguousarray(xf)).cuda()
+for c in range(3):
+    blk = np.ascontiguousarray(xf[:, c * N * 2:(c + 1) * N * 2])
+    if c == 0:
+        eng.submit(blk, N)
+    elif c == 1:
+        eng.submit_v(list(blk), N)
+    else:
+        eng.submit_device(xd.data_ptr() + c * N * 2, N * 4, N, rows=B)
+print("two tunings per input messages", len(eng.poll()))
+eng.close()
 print("sanitizer workload done")
